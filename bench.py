@@ -3,12 +3,13 @@
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference]
                     [--workload cfg2|cfg1|cfg3|cfg4|stress_dot|stress_hero] [--no-also]
+                    [--dump-outputs DIR]
 
 A *step* is one pass of the hot path over one batch of synthetic frame tuples: one
 ``FeatureVolumeManager.forward`` (hero, metadata-MLP matching) or ``CostVolumeManager.forward``
 (dot) call.  The DEFAULT workload is the hero model at 8 frames per GPU, 1 ref + 7 source
 views, 640x480 frames -> 120x160 matching maps, D = 64: at N = 1 that is BASELINE.json
-``configs[2]`` (batch 8 on one B200) and at N = 8 it is ``configs[4]`` (batch 64 over 8 GPUs, the
+``configs[2]`` (batch 8 on one H100) and at N = 8 it is ``configs[4]`` (batch 64 over 8 GPUs, the
 1/2/4/8 scaling curve).  The dot-product configuration the metric was first quoted on
 (``configs[1]``, batch 4) is measured in the same run and reported under ``"also"``.
 With N GPUs every rank processes its own batch (frames are independent: weak scaling, no
@@ -16,20 +17,22 @@ data-path collective); NCCL is used for the barrier and the MAX-reduce of the el
 
 Prints ONE JSON line (rank 0).  Keys beyond the base contract:
   roofline      hero: bound "tensor" — algorithmic MLP FLOPs per sweep launch / measured launch
-                time against MEASURED_PEAKS.json bf16_tflops_sustained (the kernel is timed inside
-                a long loop); `issued_mma` = the same with the three fp16 MMAs per product the
-                hi/lo split issues; `hbm` = the algorithmic-bytes fraction the metric asks for.
-                dot: bound "hbm" + `binding` (the on-chip gather path that actually bounds it,
-                against the MEASURED L1 ceiling of scripts/probes/l1_gather_probe).
-                `traffic` = ncu dram bytes per launch cited from profiles/ (`traffic_source`).
+                time against MEASURED_PEAKS.json bf16_tflops_sustained when present, else the H100
+                SXM data-sheet peak (`peak_source` says which); `issued_mma` = the same with the three
+                fp16 MMAs per product the hi/lo split issues; `hbm` = the algorithmic-bytes fraction.
+                dot: bound "hbm".
   cpu_baseline  the oracle's reference-structured port (oracle/costvolume_oracle.py,
                 sampler="aten": the reference's op sequence) timed on the host cores
   e2e           same metric through the public manager API with HOST (pinned) inputs
                 and outputs: H2D + sweep + D2H inside the timed region; median of 3 windows
 `--impl reference` times the CPU port alone on the SAME config (the reference is pure
-Python/PyTorch and /root/reference does not travel to the GPU box; the port is op-for-op the
-reference's own sequence and is pinned bit-exact against it in tests/test_oracle_vs_reference.py);
+Python/PyTorch; the port is op-for-op the reference's own sequence and is pinned against its
+stored outputs in tests/test_oracle_vs_reference.py);
 each step is a bounded sample of the batch (stated in `cpu_baseline.sample`), the metric is per frame.
+
+`--dump-outputs DIR` writes what the last timed step returned as DIR/<workload>_<name>.npy (float32;
+seeded inputs, so two builds can be compared output for output).  An array above its share of 64 MB
+is a fixed seeded sample, its flat indices in DIR/<workload>_<name>_index.npy.
 """
 from __future__ import annotations
 
@@ -51,17 +54,12 @@ import torch  # noqa: E402
 
 METRIC = "cost_volume_frames_per_sec@640x480_D64_K7src"
 UNIT = "frames/s"
-L2_BYTES = 126 * 1024 * 1024
+L2_BYTES = 50 * 1024 * 1024          # H100 SXM
+DUMP_BUDGET_BYTES = 64 * 10**6
 DEFAULT_WORKLOAD = "cfg2"
 ALSO_WORKLOAD = "cfg1"
 # frames per GPU (weak scaling): the single-GPU configuration's batch
 PER_GPU = {"cfg0": 1, "cfg1": 4, "cfg2": 8, "cfg3": 4, "cfg4": 8}
-# measured by scripts/probes/l1_gather_probe on a B200 (profiles/r02_l1_gather_probe.jsonl):
-# bytes the LSU/L1 path delivers to the dot sweep's exact load shape (warp-wide LDG.128 of
-# 256-byte row segments) per clock and SM at 16 / 32 / 64 resident warps
-L1_GATHER_B_PER_CLK_SM = {16: 127.6, 32: 145.0, 64: 194.4}
-
-
 def algorithmic_bytes_per_frame(w, hero: bool, with_mask: bool) -> int:
     """SURVEY.md §8(d): compulsory HBM traffic of one reference frame."""
     HW = w.height * w.width
@@ -74,8 +72,8 @@ def algorithmic_bytes_per_frame(w, hero: bool, with_mask: bool) -> int:
 
 def mlp_flops_per_frame(w, issued: bool) -> float:
     """SURVEY.md §8(d): 2 * D * HW * (F*128 + 128*128 + 128) algorithmic; `issued` counts what the
-    tcgen05 kernel actually issues: layer-1 K = 192 (the 21 pose measures enter as a per-frame bias,
-    182 live positions padded to 12 K-steps), three fp16 MMAs per product, layer 3 on SIMT."""
+    wgmma kernel actually issues: layer-1 K = 192 (the 21 pose measures enter as a per-frame bias,
+    180 live positions padded to 12 K-steps), three fp16 MMAs per product, layer 3 on SIMT."""
     rows = w.planes * w.height * w.width
     f_in = w.channels * (w.views + 1) + 10 * w.views + 4
     if issued:
@@ -90,32 +88,17 @@ def load_peaks():
         return {"hbm_gbs": float(d["hbm_gbs"]), "tf_burst": float(d["bf16_tflops"]),
                 "tf_sustained": float(d.get("bf16_tflops_sustained", d["bf16_tflops"])),
                 "source": "measured (MEASURED_PEAKS.json)"}
-    return {"hbm_gbs": 6650.0, "tf_burst": 1590.0, "tf_sustained": 1400.0,
-            "source": "fallback (B200_PROFILING.md)"}
+    return {"hbm_gbs": 3350.0, "tf_burst": 989.0, "tf_sustained": 989.0,
+            "source": "H100 SXM data sheet (3.35 TB/s HBM3, 989 TFLOP/s dense fp16 at 700 W); not reached"}
 
 
-def load_traffic(tag: str):
-    """dram bytes per launch of the dominant kernel, cited from a committed ncu summary."""
-    p = ROOT / "profiles" / "ncu_traffic.json"
-    if p.is_file():
-        try:
-            d = json.loads(p.read_text())
-            return d.get(tag), d.get("_source", {}).get(tag, "profiles/ncu_traffic.json")
-        except Exception:
-            return None, None
-    return None, None
-
-
-def make_roofline(w, hero, frames, sweep_s, prep_s, step_s, variant, sm_mhz):
+def make_roofline(w, hero, frames, sweep_s, prep_s, step_s, variant):
     pk = load_peaks()
     alg_bytes = algorithmic_bytes_per_frame(w, hero, True) * frames
     gbs = alg_bytes / sweep_s / 1e9
-    traffic, tsrc = load_traffic(f"{w.kind}:{variant}")
     common = {
         "kernel": variant, "sweep_us_per_launch": sweep_s * 1e6, "prep_us_per_launch": prep_s * 1e6,
         "sweep_share_of_step": sweep_s / step_s, "peak_source": pk["source"],
-        "traffic": traffic, "traffic_source": (f"cited from {tsrc} (one ncu --set full capture of this kernel at this "
-                                               "batch; not re-measured by this run)") if traffic else None,
         "algorithmic_bytes_per_launch": alg_bytes,
     }
     hbm = {"achieved": gbs, "peak": pk["hbm_gbs"], "unit": "GB/s", "frac": gbs / pk["hbm_gbs"]}
@@ -134,21 +117,9 @@ def make_roofline(w, hero, frames, sweep_s, prep_s, step_s, variant, sm_mhz):
             "note": ("the metadata-MLP sweep is a dense contraction at ~7000 FLOP/B: tensor-bound; the HBM "
                      "fraction the metric names is reported under `hbm`"),
         }
-    sm = 148
-    clk = (sm_mhz or 1965) * 1e6
-    samples = frames * w.planes * w.views * w.height * w.width
-    gather = samples * 4 * w.channels * 4
-    ceil64 = L1_GATHER_B_PER_CLK_SM[64]
     return {
         "bound": "hbm", **hbm, **common,
-        "binding": {"resource": "l1_gather_bytes", "achieved_B_per_clk_sm": gather / sweep_s / clk / sm,
-                    "peak_B_per_clk_sm": ceil64, "frac": gather / sweep_s / clk / sm / ceil64,
-                    "peak_source": ("measured: scripts/probes/l1_gather_probe, this load shape, 64 warps/SM "
-                                    f"(16 warps: {L1_GATHER_B_PER_CLK_SM[16]}, 32: {L1_GATHER_B_PER_CLK_SM[32]}); "
-                                    "profiles/r02_l1_gather_probe.jsonl"),
-                    "sm_mhz_used": sm_mhz or 1965},
-        "note": ("HBM fraction as the metric demands; at 116 FLOP/B the dot sweep is bound by the on-chip "
-                 "gather path — see `binding` and DESIGN.md"),
+        "note": "HBM fraction of the algorithmic bytes; at 116 FLOP/B the dot sweep is bound on chip (DESIGN.md)",
     }
 
 
@@ -313,7 +284,7 @@ def workload_config(w, batch_per_gpu, world):
         "feature_map": f"{w.width}x{w.height}", "planes": w.planes, "src_views": w.views,
         "channels": w.channels, "batch_per_gpu": batch_per_gpu, "global_batch": batch_per_gpu * world,
         "parallelism": f"frame-sharded x{world} (no data-path collective)",
-        "l2": (f"{n_sets} rotating input sets, {n_sets * in_bytes / 2**20:.0f} MiB > 126 MiB L2; "
+        "l2": (f"{n_sets} rotating input sets, {n_sets * in_bytes / 2**20:.0f} MiB > 50 MiB L2; "
                f"outputs ({4 * batch_per_gpu * w.planes * w.height * w.width / 2**20:.0f} MiB/step) freshly allocated"),
     }, n_sets
 
@@ -413,10 +384,13 @@ def measure_gpu(w, per_gpu, steps, warmup, dev, rank, world, sampler, S, _native
         sampler.active.set()
         e0.record()
         for i in range(steps):
-            step(i)
+            last = step(i)
         e1.record()
         torch.cuda.synchronize()
         sampler.active.clear()
+        names = ("cost_volume", "lowest_cost_depth", "depth_planes", "overall_mask")
+        outputs = {n: v.float().cpu() for n, v in zip(names, last) if v is not None}
+        del last
         sharding.barrier()
         ms_local = e0.elapsed_time(e1)
         launches = _native.launch_count() - launches0
@@ -465,15 +439,31 @@ def measure_gpu(w, per_gpu, steps, warmup, dev, rank, world, sampler, S, _native
     rec = {
         "value": frames_step * steps / (ms_total * 1e-3), "ms_per_step": ms_total / steps, "config": cfg,
         "roofline": make_roofline(w, hero, per_gpu, sweep_s, prep_ms * 1e-3 / max(nrec, 1),
-                                  ms_local * 1e-3 / steps, variant, clocks.get("sm_mhz")),
+                                  ms_local * 1e-3 / steps, variant),
         "e2e": {"value": frames_step * e2e_steps / (e2e_ms * 1e-3), "unit": UNIT, "h2d_bytes_per_step": h2d,
                 "d2h_bytes_per_step": d2h, "steps": e2e_steps, "ms_per_step": e2e_ms / e2e_steps,
                 "windows_ms_per_step": [x / e2e_steps for x in windows],
                 "mode": ("HostStreamer: H2D(i+1) || sweep(i) || D2H(i-1) on three streams, pinned host buffers, "
                          "persistent device input ring; median of 3 windows")},
-        "gpu_launches": launches, "clocks": clocks, "kernel_variant": variant,
+        "gpu_launches": launches, "clocks": clocks, "kernel_variant": variant, "outputs": outputs,
     }
     return rec
+
+
+def dump_outputs(out_dir, per_workload):
+    """Writes {workload: {name: cpu tensor}} as float32 .npy files; see the module docstring."""
+    import numpy as np
+    out = Path(out_dir)
+    out.mkdir(parents=True, exist_ok=True)
+    arrays = [(f"{wname}_{n}", t) for wname, d in per_workload.items() for n, t in d.items()]
+    cap = DUMP_BUDGET_BYTES // (12 * max(len(arrays), 1))    # elements: 4 B value + 8 B index per sample
+    for name, t in arrays:
+        if t.numel() > cap:
+            g = torch.Generator().manual_seed(0)
+            idx = torch.randperm(t.numel(), generator=g)[:cap].sort().values
+            np.save(out / f"{name}_index.npy", idx.to(torch.float64).numpy())
+            t = t.reshape(-1)[idx]
+        np.save(out / f"{name}.npy", t.numpy().astype(np.float32))
 
 
 def main():
@@ -486,6 +476,8 @@ def main():
     ap.add_argument("--variant", default="auto", choices=["auto", "generic", "fast"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-also", action="store_true", help="skip the secondary (dot cfg1) record")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<workload>_<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
 
@@ -531,6 +523,9 @@ def main():
         line["also"] = {wa.name: {k: ra[k] for k in ("value", "ms_per_step", "config", "roofline", "e2e",
                                                      "gpu_launches", "clocks", "kernel_variant")}}
     sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {w.name: rec["outputs"],
+                                         **({wa.name: ra["outputs"]} if "also" in line else {})})
 
     if rank == 0 and world == 1 and not args.no_cpu_baseline:
         if full_affinity is not None:

@@ -1,5 +1,5 @@
 /*
- * srcv_b200 — C ABI of the B200-native plane-sweep cost-volume library.
+ * srcv_b200 — C ABI of the H100-native plane-sweep cost-volume library.
  *
  * This is the drop-in boundary for SimpleRecon's cost-volume hot path.  The
  * reference has no native layer (it is pure PyTorch), so each entry point below
@@ -39,7 +39,7 @@ typedef enum srcv_status {
   SRCV_ERR_WORKSPACE = 3,   /* workspace too small or misaligned               */
   SRCV_ERR_UNSUPPORTED = 4, /* valid request this build cannot serve           */
   SRCV_ERR_CUDA = 5,        /* CUDA runtime error (see srcv_last_error)        */
-  SRCV_ERR_DEVICE = 6       /* current device is not an sm_100 part            */
+  SRCV_ERR_DEVICE = 6       /* current device is not an sm_90 part             */
 } srcv_status;
 
 /* Problem shape.  Mirrors the tensor contract of
@@ -173,7 +173,7 @@ int32_t srcv_dot_backward_f32(const srcv_shape* shape, const float* cur_feats, c
 /* ---- single-plane warp -------------------------------------------------- *
  * Replaces CostVolumeManager.warp_features (reference modules/cost_volume.py:139-234),
  * the helper that MATERIALISES the warped source features of one depth plane; the
- * sweeps above never call it (they keep the warped values in registers / TMEM), it is
+ * sweeps above never call it (they keep the warped values in registers / shared memory), it is
  * exported because the reference exposes it as a method.  shape->D is ignored.
  *   depth_plane  DEVICE (B) one depth per frame, or (B,H,W) when per_pixel != 0
  *   warped (B,K,C,H,W)  depths (B,K,H,W) = z' of the plane point in each source camera
@@ -357,7 +357,7 @@ int32_t srcv_mvloss_backward_f32(const srcv_mvloss_args* args, const float* grad
 typedef enum srcv_variant {
   SRCV_VARIANT_AUTO = 0,
   SRCV_VARIANT_GENERIC = 1, /* shape-generic SIMT kernels                     */
-  SRCV_VARIANT_FAST = 2     /* chunk-planar gather / tcgen05 kernels          */
+  SRCV_VARIANT_FAST = 2     /* chunk-planar gather / wgmma kernels            */
 } srcv_variant;
 int32_t srcv_set_variant(int32_t variant);
 /* Name of the kernel variant the last forward call on this process launched. */
@@ -368,7 +368,7 @@ uint64_t srcv_launch_count(void);
 
 /* ---- tensor-core self-test (test support) -------------------------------- *
  * D (128,128) = A (128,Kp) W^T, W (128,Kp), all DEVICE fp32, Kp a multiple of 16
- * and <= 256, through the same TMEM / descriptor / mbarrier machinery as the
+ * and <= 256, through the same descriptors and (hi, lo) split as the
  * metadata-MLP kernel (fp16 hi/lo split, three MMAs).  `scratch` = 512*Kp bytes.  */
 int32_t srcv_tc_selftest_f32(const float* A, const float* W, int32_t Kp, float* D, void* scratch,
                              void* stream);

@@ -7,8 +7,8 @@ library is missing instead of falling back to anything in here.
 
 Parity pin: the reference holds no tests or golden vectors for this path
 (SURVEY.md §8c), so this restatement is pinned against the *reference's own classes*
-imported from ``/root/reference`` in the build container (``oracle/ref_import.py``)
-— live in ``tests/test_oracle_vs_reference.py`` and through the committed fixtures
+(imported unmodified by ``oracle/ref_import.py``) through their stored outputs —
+``tests/test_oracle_vs_reference.py`` (``tests/golden/reference/``) and the committed fixtures
 ``tests/golden/*.npz`` made by ``tests/golden/make_golden.py``.
 
 What is restated (all citations relative to the reference tree):

@@ -1,11 +1,12 @@
-"""Import the UNMODIFIED reference classes from /root/reference (build container only).
+"""Import the UNMODIFIED reference classes from the SimpleRecon source tree named by
+``$SIMPLERECON_REF``.
 
 TEST INFRASTRUCTURE — never imported by the product package.
 
-The reference tree is read-only and absent on the GPU box, so this module is used
-only (a) by ``tests/golden/make_golden.py`` to generate the committed golden
-vectors and (b) by ``-m "not gpu"`` tests that pin the oracle against the live
-reference when ``/root/reference`` happens to exist.
+The tests never need the reference tree: this module is used by the scripts under
+``tests/golden/`` that generate the committed golden vectors and stored reference outputs,
+and by the two tests of ``install()`` against the real reference modules, which skip
+without it.
 
 Why stubs: ``modules/cost_volume.py`` itself needs only torch + einops, but its
 imports pull ``modules/networks.py:1,4`` (antialiased_cnns, timm),
@@ -24,15 +25,12 @@ import sys
 import types
 
 REF_ENV = "SIMPLERECON_REF"
-_DEFAULT_ROOTS = ("/root/reference",)
 
 
 def reference_root() -> str | None:
-    cands = [os.environ.get(REF_ENV)] if os.environ.get(REF_ENV) else []
-    cands += list(_DEFAULT_ROOTS)
-    for c in cands:
-        if c and os.path.isfile(os.path.join(c, "modules", "cost_volume.py")):
-            return c
+    c = os.environ.get(REF_ENV)
+    if c and os.path.isfile(os.path.join(c, "modules", "cost_volume.py")):
+        return c
     return None
 
 
@@ -72,7 +70,7 @@ def load_reference():
     root = reference_root()
     if root is None:
         raise RuntimeError(
-            "reference tree not found (set $SIMPLERECON_REF or mount /root/reference)"
+            "reference tree not found (set $SIMPLERECON_REF to the SimpleRecon source tree)"
         )
     _install_stubs()
     if root not in sys.path:
@@ -118,7 +116,7 @@ def load_reference_tsdf():
         return _cached_tsdf
     root = reference_root()
     if root is None:
-        raise RuntimeError("reference tree not found (set $SIMPLERECON_REF or mount /root/reference)")
+        raise RuntimeError("reference tree not found (set $SIMPLERECON_REF to the SimpleRecon source tree)")
     for name in ("trimesh", "skimage", "skimage.measure"):
         if name not in sys.modules:
             sys.modules[name] = types.ModuleType(name)

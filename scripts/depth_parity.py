@@ -1,20 +1,15 @@
 """Depth-map parity through the reference's own U-Net (BASELINE target: depth Abs-Diff <= 1e-4).
 
-The reference's `CVEncoder` + `DepthDecoderPP` (reference modules/networks.py:20-127) turn a
-cost volume + image-prior features into the depth map.  They live only in /root/reference
-(build container, CPU); our kernels run only on the GPU box.  So the check has two halves:
-
-    # on the GPU box (through gpurun): our cost volumes for seeded 640x480 tuples
-    python scripts/depth_parity.py dump        ->  gpurun_out/depth_parity_ours.npz
-
-    # in the build container: reference cost volumes (CPU, reference classes) for the SAME
-    # tuples, then the reference decoder on both, Abs-Diff of depth_pred_s0_b1hw
-    python scripts/depth_parity.py eval        ->  profiles/depth_parity_r02.json
+The reference's `CVEncoder` + `DepthDecoderPP` (reference modules/networks.py:20-127) turn a cost
+volume into the depth map; they exist only in the SimpleRecon tree ($SIMPLERECON_REF).  Two halves:
+`dump` (GPU: our volumes for seeded 640x480 tuples -> $SRCV_DEPTH_PARITY_DUMP, default in the temp
+dir) and `eval` (the reference's volumes for the same tuples, both through its decoder, Abs-Diff of
+depth_pred_s0_b1hw -> $SRCV_DEPTH_PARITY_REPORT).
 
 Round 2: a BATCH per model — 8 hero frames (one B = 8 call, BASELINE configs[2]'s shard) and 4
 dot frames (configs[1]) at 640x480 — with the Abs-Diff reported per frame.  The two halves are
-also tests: tests/test_gpu_depth_parity.py writes the dump on the GPU box, tests/test_depth_parity_eval.py
-evaluates it here when both the dump and /root/reference are present.
+also tests: tests/test_gpu_depth_parity.py writes the dump on the GPU, tests/test_depth_parity_eval.py
+evaluates it when both the dump and the reference tree are present.
 
 Seeded random weights everywhere (no checkpoint exists in this environment, SURVEY.md §8c);
 image-prior pyramid = seeded random tensors with EfficientNetV2-S channel counts
@@ -24,7 +19,9 @@ image-prior pyramid = seeded random tensors with EfficientNetV2-S channel counts
 from __future__ import annotations
 
 import json
+import os
 import sys
+import tempfile
 from pathlib import Path
 
 import numpy as np
@@ -37,9 +34,9 @@ from simplerecon_b200.synthetic import make_tuple, mlp_state  # noqa: E402
 
 H, W, D, K, C = 120, 160, 64, 7, 16
 SEEDS = {"dot": 2024, "hero": 2025}
-FRAMES = {"dot": 4, "hero": 8}          # 4 x 19.7 MB + 8 x 4.9 MB... fp32 volumes: 59 MB < gpurun_out's 64 MiB
-DUMP = ROOT / "gpurun_out" / "depth_parity_ours.npz"
-REPORT = ROOT / "profiles" / "depth_parity_r02.json"
+FRAMES = {"dot": 4, "hero": 8}          # 4 x 19.7 MB + 8 x 4.9 MB fp32 volumes: 59 MB
+DUMP = Path(os.environ.get("SRCV_DEPTH_PARITY_DUMP", Path(tempfile.gettempdir()) / "srcv_depth_parity_ours.npz"))
+REPORT = Path(os.environ.get("SRCV_DEPTH_PARITY_REPORT", Path(tempfile.gettempdir()) / "srcv_depth_parity.json"))
 
 
 def dump():

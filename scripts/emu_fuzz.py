@@ -23,7 +23,7 @@ from tests.parity import cost_tol  # noqa: E402
 def rand_case(g, kind):
     ri = lambda a, b: int(torch.randint(a, b + 1, (1,), generator=g))
     B, K = ri(1, 2), ri(1, 8 if kind.startswith("dot") else 7)
-    if kind == "tc":                        # the tcgen05 kernel's layout
+    if kind == "tc":                        # the wgmma kernel's layout
         K = 7
     C = [8, 16, 16, 16, 12][ri(0, 4)] if kind == "dot" else ([8, 16, 16][ri(0, 2)])
     if kind == "tc":

@@ -7,7 +7,7 @@
 // arithmetic beyond keeping the values alive, and reports bytes per clock per SM, so that the
 // sweep's achieved L1 rate has a MEASURED denominator next to the nominal 128 B/clk/SM.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/probes/l1_gather_probe scripts/probes/l1_gather_probe.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/probes/l1_gather_probe scripts/probes/l1_gather_probe.cu
 //   ./scripts/probes/l1_gather_probe            (prints one JSON line per access shape)
 #include <cstdio>
 #include <cstdlib>

@@ -1,8 +1,8 @@
-"""simplerecon_b200 — B200-native plane-sweep cost volume behind SimpleRecon's
+"""simplerecon_b200 — H100-native plane-sweep cost volume behind SimpleRecon's
 ``CostVolumeManager`` / ``FeatureVolumeManager`` API.
 
 Only the hot path named by BASELINE.json is here: the cost-volume build of the
-reference's ``modules/cost_volume.py``, as hand-written sm_100a kernels in
+reference's ``modules/cost_volume.py``, as hand-written sm_90a kernels in
 ``csrc/`` behind a C ABI (``include/srcv_b200.h``), plus the Python mirror of the
 reference's manager classes that binds it.  Encoders, decoder, datasets and
 training stay the reference's own PyTorch code.

@@ -136,7 +136,7 @@ def load() -> C.CDLL:
     if not path.is_file():
         raise NativeLibraryError(
             f"{path} not found — build it with `python -m simplerecon_b200.build` "
-            "(nvcc, sm_100a).  There is no CPU or PyTorch fallback for this path.")
+            "(nvcc, sm_90a).  There is no CPU or PyTorch fallback for this path.")
     lib = C.CDLL(str(path))
     for name, (res, args) in SYMBOLS.items():
         try:

@@ -1,10 +1,10 @@
-"""Builds ``lib/libsrcv_b200.so`` in-tree with nvcc for sm_100a.
+"""Builds ``lib/libsrcv_b200.so`` in-tree with nvcc for sm_90a.
 
     python -m simplerecon_b200.build [--force] [--verbose]
 
 Plain ``nvcc -shared`` (no torch headers: the library is a C ABI, torch only
-supplies device memory and streams at run time).  The .so is git-ignored but
-travels with the working tree to the GPU box.
+supplies device memory and streams at run time).  The .so is a build product
+(git-ignored); ``__graft_entry__.build()`` recreates it when a source is newer.
 """
 from __future__ import annotations
 
@@ -22,7 +22,7 @@ HDR = sorted((PKG / "csrc").glob("*.cuh")) + sorted((PKG / "csrc").glob("*.h")) 
 OUT = PKG / "lib" / "libsrcv_b200.so"
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",
 ]
 # Preprocessor switches of the shipped build.  tests/emu compiles the same sources with the same

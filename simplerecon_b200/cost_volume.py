@@ -1,4 +1,4 @@
-"""Drop-in cost-volume managers backed by the sm_100a kernels.
+"""Drop-in cost-volume managers backed by the sm_90a kernels.
 
 Class names, constructor signatures, method names, ``forward`` signature / return
 tuple, buffers and ``state_dict`` keys follow the reference's
@@ -29,7 +29,7 @@ def _require_cuda(dev) -> None:
     host-emulated library; the product never bypasses it.)"""
     if dev.type != "cuda":
         raise RuntimeError(
-            "simplerecon_b200 cost volumes run on CUDA (sm_100a) only; got tensors on "
+            "simplerecon_b200 cost volumes run on CUDA (sm_90a) only; got tensors on "
             f"{dev}.  There is no CPU fallback.")
 
 
@@ -156,7 +156,7 @@ class _DotVolumeFunction(torch.autograd.Function):
 
 
 class _MlpVolumeFunction(torch.autograd.Function):
-    """Differentiable wrapper of the metadata-MLP sweep: fused forward (tcgen05 where the
+    """Differentiable wrapper of the metadata-MLP sweep: fused forward (wgmma where the
     shape allows), and ``srcv_mlp_backward_f32`` — a recompute kernel, nothing but the inputs
     is saved — for the two feature inputs and the six MLP parameters: what autograd of the
     reference composite (modules/cost_volume.py:451-736, modules/networks.py:129-147) yields.
@@ -479,7 +479,7 @@ class FeatureVolumeManager(CostVolumeManager):
                            + 3 * num_source_views)                       # pose measures
         self.mlp = MLP(channel_list=mlp_channels, disable_final_activation=True)
         print(f" simplerecon_b200 {self._banner}: {num_source_views} source views, "
-              f"MLP channels {mlp_channels} (sm_100a fused sweep) ")
+              f"MLP channels {mlp_channels} (sm_90a fused sweep) ")
 
     def _mlp_weights(self, dev, n_features):
         lin = [m for m in self.mlp.net if isinstance(m, nn.Linear)]

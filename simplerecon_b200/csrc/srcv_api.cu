@@ -118,7 +118,7 @@ int32_t srcv_check_device(void) {
   int major = 0;
   e = cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev);
   if (e != cudaSuccess) return cuda_fail(e, "cudaDeviceGetAttribute");
-  if (major != 10) return fail(SRCV_ERR_DEVICE, "device %d has compute capability %d.x; this library is built for sm_100a only", dev, major);
+  if (major != 9) return fail(SRCV_ERR_DEVICE, "device %d has compute capability %d.x; this library is built for sm_90a only", dev, major);
   return SRCV_OK;
 }
 
@@ -349,7 +349,7 @@ int32_t srcv_mlp_forward_f32(const srcv_shape* s, const float* cur, const float*
   const bool per_pixel = pl->mode == SRCV_PLANES_PER_PIXEL;
   const float* planes = pl->mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl->planes;
   if (tc) {
-    g_last_variant.store("mlp_tc_tcgen05_f16x3");
+    g_last_variant.store("mlp_tc_wgmma_f16x3");
     err = launch_mlp_tc(*s, cur, ws, planes, per_pixel, *w, cost, lowest, overall_mask, stream);
   } else {
     g_last_variant.store("mlp_generic_fp32");

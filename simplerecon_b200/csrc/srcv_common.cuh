@@ -1,11 +1,11 @@
-// Shared device-side geometry for the plane-sweep kernels (sm_100a).
+// Shared device-side geometry for the plane-sweep kernels (sm_90a).
 //
 // The arithmetic restated here is the reference's
 //   BackprojectDepth.forward   utils/geometry_utils.py:51-59  (+0.5 pixel centres :34-44)
 //   Project3D.forward          utils/geometry_utils.py:72-89  (eps 1e-8)
 //   uv normalisation           modules/cost_volume.py:199, :587
 //   F.grid_sample(bilinear, zeros, align_corners=False)  modules/cost_volume.py:201-212
-// re-associated the B200 way.  The depth-invariant part of the projection,
+// re-associated for the GPU.  The depth-invariant part of the projection,
 //   Hm = (K E)[:3,:3] invK[:3,:3]   and   t = (K E)[:3,3],
 // is folded once per (frame, view) by the prep kernel in fp64, so a plane hypothesis d
 // at pixel centre p projects with three FMAs,  c = d (Hm p) + t  — the plane-induced
@@ -45,33 +45,11 @@ constexpr float kEpsNorm = 1e-12f;  // F.normalize default
 constexpr float kEpsCos = 1e-5f;    // modules/cost_volume.py:687
 constexpr float kLeaky = 0.01f;     // nn.LeakyReLU default slope
 
-// ---- packed fp32: two independent IEEE FMAs / multiplies in ONE issue slot (SASS FFMA2 / FMUL2) ----
-// Bit-identical to the two scalar operations; what they save is issue bandwidth, which is what the
-// sweeps' gather / blend loops and the epilogue warps of the tcgen05 kernel are short of.
-#ifdef SRCV_HOST_EMU
-inline float2 fma2(float2 a, float2 b, float2 c) { return float2{std::fmaf(a.x, b.x, c.x), std::fmaf(a.y, b.y, c.y)}; }
-inline float2 mul2(float2 a, float2 b) { return float2{a.x * b.x, a.y * b.y}; }
-#else
+// ---- fp32 pairs: two independent IEEE FMAs / multiplies on (even, odd) channel pairs -----------
 __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
+  return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y));
 }
-__device__ __forceinline__ float2 mul2(float2 a, float2 b) {
-  unsigned long long ra, rb, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mul.rn.f32x2 %0, %1, %2;" : "=l"(rd) : "l"(ra), "l"(rb));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
-#endif
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
 
 // Per (frame b, view k) constants, written by prep_kernel.  32 floats = 128 B.
 struct __align__(16) ViewParams {
@@ -83,8 +61,8 @@ struct __align__(16) ViewParams {
   float comb;      // pose_distance: sqrt(t_meas^2 + r_meas^2)
   float rmeas;     // sqrt(2 (1 - min(3, tr R)/3))
   float tmeas;     // |src_poses[:3,3]|
-  uint32_t rt_hi;  // (rmeas, tmeas) as the fp16 (hi, lo) operand words of the tcgen05 kernel
-  uint32_t rt_lo;  //   (csrc/srcv_tc.cuh split_pack), so the sweep does not re-split constants
+  uint32_t rt_hi;  // (rmeas, tmeas) as fp16 (hi, lo) operand words
+  uint32_t rt_lo;  //   (csrc/srcv_tc.cuh split_pack)
   float pad[12];
 };
 static_assert(sizeof(ViewParams) == 128, "ViewParams must be 128 bytes");

@@ -338,7 +338,7 @@ cudaError_t launch_dot_fast(const srcv_shape& s, const float* cur, const Workspa
   // sweep is latency-bound at low occupancy and smaller CTAs balance better: measured
   // 428 -> 370 us at B = 4); the argmax of a split sweep is done by the last CTA of each
   // pixel tile to finish (see the kernel).
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   static const int tile_w = [] {

@@ -83,7 +83,7 @@ cudaError_t launch_mlp_backward(const srcv_shape& s, const float* cur, const flo
                                 const srcv_mlp_weights& w, const float* gcost, float* gcur,
                                 float* gsrc, const srcv_mlp_grads& g, cudaStream_t stream);
 
-// tensor-core variant (tcgen05): K = 7, C = 16, 202 -> 128 -> 128 -> 1
+// tensor-core variant (wgmma): K = 7, C = 16, 202 -> 128 -> 128 -> 1
 bool mlp_tc_supported(const srcv_shape& s, const srcv_mlp_weights& w);
 size_t mlp_tc_extra_bytes(const srcv_shape& s);
 size_t mlp_tc_image_bytes();

@@ -465,7 +465,7 @@ cudaError_t launch_mlp_backward(const srcv_shape& s, const float* cur, const flo
   note_launch();
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return err;
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 1;
   if (cudaGetDevice(&dev) == cudaSuccess) cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const long long n_tiles = (long long)s.B * s.D * ((s.H * s.W + BT - 1) / BT);
   const int grid = (int)(n_tiles < sms ? n_tiles : sms);     // one persistent CTA per SM

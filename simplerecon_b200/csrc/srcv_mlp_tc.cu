@@ -1,41 +1,24 @@
-// Metadata-MLP plane-sweep volume on the 5th-generation tensor cores (tcgen05).
+// Metadata-MLP plane-sweep volume on the Hopper tensor cores (wgmma).
 //
 // Replaces FeatureVolumeManager / FastFeatureVolumeManager.build_cost_volume
 // (reference modules/cost_volume.py:451-736, :967-1164) for the hero layout
 // K = 7 source views, C = 16 channels, MLP 202 -> 128 -> 128 -> 1.
 //
-// One persistent CTA per SM walks over row tiles; a tile = 128 rows = a 16 x 2 patch of
-// pixels at four consecutive depth planes.  Warp roles (640 threads):
-//   * 12 BUILDER warps, three threads per row: project, gather (chunk-planar copies of the
-//     features, csrc/srcv_prep.cu), blend on packed fp32 pairs (FFMA2) and build the row's metadata
-//     channels in registers, split every value into an fp16 (hi, lo) pair and write them straight
-//     into TENSOR MEMORY as the A operand (tcgen05.st) — the (B,F,H,W) / (B*D,H,W,F) tensors the
-//     reference materialises exist only as 192 TMEM columns per row.  Two whole views per thread,
-//     then half of view 2 (slots 0, 1) or the tail (slot 2);
-//   * 1 MMA-issuing thread (elect.sync): layer 1 = 12 x 3 tcgen05.mma (A from TMEM, weights from
-//     shared memory, fp32 accumulator in TMEM):  A_hi W_hi + A_hi W_lo + A_lo W_hi, issued as two
-//     64-column halves; the WHOLE layer-1 bias rides in the MMA — a constant-one K position against
-//     a weight row holding 16 (b1 + the frame's pose-measure contribution), which this warp rewrites
-//     in shared memory when its tiles move on to another frame; layer 2 = 8 x 3 tcgen05.mma in two
-//     K halves, accumulating into the first 128 columns of the tile's own (by then dead) A1 buffer;
-//   * 4 EPILOGUE warps, one thread per row: after each layer-1 half they read the accumulator,
-//     apply LeakyReLU, split to fp16 (hi, lo) and write the layer-2 A operand back IN PLACE (a
-//     chunk's 32 fp32 columns become its 16 hi + 16 lo operand columns, so nothing else is
-//     touched); after layer 2 they apply bias + LeakyReLU and the 128 -> 1 layer as one dot
-//     product per row (packed FFMA2 chains) and store the cost.
-// Stages are chained by mbarriers (tcgen05.commit for MMA completion).  The roles overlap: with two
-// A1 buffers the builders gather tile t+1 while the epilogue warps post-process tile t and the
-// tensor pipe runs its MMAs; the layer-1 MMAs of tile t+1 start while the layer-2 epilogue of tile
-// t is still running; within a tile the epilogue of one half overlaps the MMAs of the other.
-// Weights (both layers, hi and lo, 164 KB) stay resident in shared memory for the CTA's lifetime,
-// laid out as K-major no-swizzle core matrices by the pack kernel.
+// One persistent CTA per SM walks over 64-row tiles (a 16 x 2 pixel patch at two consecutive planes):
+//   * 8 BUILDER warps (four threads per row, two K blocks each) project, gather, blend, build the
+//     metadata channels and write the row's fp16 (hi, lo) layer-1 operand into a 48 KB shared tile;
+//   * 2 CONSUMER warpgroups take tiles in turn: layer 1 = 12 x 3 wgmma m64n128k16 (A_hi W_hi + A_hi W_lo
+//     + A_lo W_hi), after which the tile goes back to the builders; the layer-1 accumulator fragment,
+//     biased, LeakyReLU'd and split in registers, IS the register A operand of layer 2 (8 x 3 wgmma
+//     m64n64k16 per 64-column half); the 128 -> 1 layer is a per-row dot product reduced over a quad.
+// Stages are chained by mbarriers; weights (160 KB, K-major no-swizzle core matrices) stay resident in
+// shared memory, pulled in once by the bulk-copy engine.
 //
 // The K order of layer 1 is OURS (the pack kernel permutes W1's columns to match), 8 blocks x 24:
 //   per view k:  16 warped | mask | z' | dot | ray angle | n_src (3) | pad
-//     (view 2, built by two threads:  8 warped | dot | mask | z' | angle || 8 warped | dot | n_src (3))
-//   tail:        16 reference features | plane depth | n_cur (3) | ONE (bias) | pad
-// The 21 pose measures (comb, r, t per view) are constant per (frame, view) and enter through the
-// bias row instead of 21 K positions.
+//   tail:        16 reference features | plane depth | n_cur (3) | pad (4)
+// The 21 pose measures (comb, r, t per view) are constant per (frame, view) and enter, with b1, as a
+// per-frame bias vector instead of 21 K positions.
 //
 // Scaling: W1 and W2 are stored x16 (exact) so the lo halves of typical |w| ~ 0.05 weights
 // stay out of the fp16 subnormals.  Layer 1 therefore yields 16 (W1 x + b1); LeakyReLU
@@ -50,87 +33,52 @@ namespace {
 
 using namespace tc;
 
+#ifndef SRCV_TC_REGS_BUILD
+#define SRCV_TC_REGS_BUILD 96
+#endif
+
 constexpr int kC = 16, kViews = 7;
-constexpr int kRows = 128;               // rows (TMEM lanes) per tile
-// A tile is a 16 x 2 pixel patch at FOUR consecutive depth planes (32 pixels x 4 planes =
-// 128 rows): warp w of a lane group works plane w of the same patch, so the four warps'
-// gathers for one source view walk along the same epipolar lines and share L1 lines.
-constexpr int kTileW = 16, kTileH = 2, kTileD = 4;
+constexpr int kRows = 64;                // rows (M of one wgmma) per tile
+// A tile is a 16 x 2 pixel patch at TWO consecutive depth planes (32 pixels x 2 planes = 64 rows):
+// the builder warps of both planes gather along the same epipolar lines and share L1 lines.
+constexpr int kTileW = 16, kTileH = 2, kTileD = 2;
 constexpr int kN = 128;                  // layer widths
-constexpr int kBlk = 24;                 // K positions per block (23 per view + 1 pad; tail 21 + 3 pad)
+constexpr int kBlk = 24;                 // K positions per block (23 per view + 1 pad; tail 20 + 4 pad)
 constexpr int kBlkCols = kBlk / 2;       // 12 packed columns per block and half
 constexpr int kK1 = 192;                 // 8 blocks x 24  (12 k-steps of 16)
 constexpr int kK2 = 128;
 constexpr int kF = kC * (kViews + 1) + 10 * kViews + 4;  // 202
-constexpr int kBiasPos = kViews * kBlk + kC + 4;         // K position of the constant one
-
-// TMEM columns (32-bit): two K elements per column.  TWO A1 buffers (tile t uses buffer t & 1), so
-// the builders run a whole tile ahead of the tensor pipe; the layer-2 accumulator D2 of tile t
-// lands in the first 128 columns of tile t's own A1 buffer, which is dead once its layer-1 MMAs
-// are done.   A1[0]: hi 0..95 | lo 96..191    A1[1]: 192..383    DA: 384..511
-constexpr uint32_t kColA1 = 0, kA1Stride = kK1, kA1LoOff = kK1 / 2, kColDA = 2 * kK1, kTmemCols = 512;
-static_assert(kColDA + kN <= kTmemCols, "TMEM budget");
-static_assert(kN <= kK1, "D2 must fit in an A1 buffer");
 
 constexpr float kWScale = 16.0f;
 constexpr float kUnscale2 = 1.0f / (kWScale * kWScale);
 
-// Warps 0-11 build, 12-15 run the epilogues, 16 issues the MMAs; 17-19 complete its warpgroup
-// (setmaxnreg works on aligned groups of four warps): the kernel is launched at 96 registers per
-// thread, the MMA group shrinks to 24, builders grow to 112 (all 16 vector loads of a bilinear
-// footprint in flight) and the epilogue group to 120.
-// setmaxnreg only REDISTRIBUTES the CTA's launch-time allocation (640 x 96 registers): an .inc
-// blocks until the pool holds enough, so the totals below must fit it or the CTA deadlocks.
-#ifdef SRCV_TC_W24
-// 24 warps: SIXTEEN builder warps (four threads per row, two K blocks each: views 2s, 2s+1; slot 3 the
-// last view and the tail), four epilogue warps, the MMA warp and its three idle group mates.  Registers
-// are allocated per four warps, so 768 threads launch at 80; the MMA group's 56 x 128 freed registers go
-// to the epilogue group (and, in the B split, to the builders).
-constexpr int kBuildWarps = 16, kEpiWarps = 4, kMmaWarp = 20;
-constexpr int kThreads = 24 * 32;
-constexpr int kSlots = 4;
-constexpr bool kSetmaxnreg = true;
-constexpr int kRegsLaunch = 80;
-#ifdef SRCV_TC_W24B
-constexpr int kRegsBuild = 88, kRegsEpi = 104, kRegsMma = 24;
-constexpr int kEpiStep = 32;
-#else
-constexpr int kRegsBuild = 80, kRegsEpi = 120, kRegsMma = 24;
-constexpr int kEpiStep = 64;
-#endif
-constexpr int kSplitView = -1;           // no view is split: 2 / 2 / 2 / 1 + tail blocks per slot
-#else
-constexpr int kBuildWarps = 12, kEpiWarps = 4, kMmaWarp = 16;
-constexpr int kThreads = 20 * 32;
-constexpr int kSlots = 3;
-#ifdef SRCV_TC_NO_SETMAXNREG
-constexpr bool kSetmaxnreg = false;
-#else
-constexpr bool kSetmaxnreg = true;
-#endif
-constexpr int kRegsLaunch = 96;          // what ptxas allocates under __launch_bounds__(640, 1)
-constexpr int kRegsBuild = 112, kRegsEpi = 120, kRegsMma = 24;
-constexpr int kEpiStep = 64;
-// The 7 view blocks + the tail do not divide by the three builder threads of a row: view kSplitView is
-// built as TWO half-view units (channels 8h..8h+7 each, see unit_issue) by slots 0 and 1, so the slots
-// carry 2.5 / 2.5 / 2 views + tail instead of 3 / 3 / 1 + tail.
-constexpr int kSplitView = 2;
-#endif
-constexpr int kBuilders = kBuildWarps * 32, kEpis = kEpiWarps * 32;
-static_assert(!kSetmaxnreg || kBuilders * kRegsBuild + kEpis * kRegsEpi + (kThreads - kBuilders - kEpis) * kRegsMma <= kThreads * kRegsLaunch,
-              "setmaxnreg budget: increases must be covered by the decreases within the CTA's launch allocation");
-static_assert(kRegsBuild % 8 == 0 && kRegsEpi % 8 == 0 && kRegsMma % 8 == 0, "setmaxnreg takes multiples of 8");
+// Warps 0-7 build (slot = warp / 2), warps 8-15 are the two consumer warpgroups.  setmaxnreg moves
+// registers from the builders to the consumers; it only REDISTRIBUTES the launch-time allocation
+// (an .inc blocks until the pool holds enough), so the totals must fit.
+constexpr int kBuildWarps = 8, kSlots = 4, kConsumers = 2;
+constexpr int kThreads = (kBuildWarps + 4 * kConsumers) * 32;
+constexpr int kBuilders = kBuildWarps * 32;
+constexpr int kRegsLaunch = 65536 / kThreads, kRegsBuild = SRCV_TC_REGS_BUILD, kRegsCons = 2 * kRegsLaunch - kRegsBuild;
+static_assert(kBuilders == kSlots * kRows, "one builder thread per (row, slot)");
+static_assert(kBuilders * kRegsBuild + (kThreads - kBuilders) * kRegsCons <= kThreads * kRegsLaunch &&
+              kRegsBuild % 8 == 0 && kRegsCons % 8 == 0 && kRegsCons <= 256, "setmaxnreg budget");
 
 // shared memory image (bytes)
 constexpr uint32_t kW1Bytes = kN * kK1 * 2, kW2Bytes = kN * kK2 * 2;   // one of (hi, lo)
 constexpr uint32_t kOffW1Hi = 0, kOffW1Lo = kW1Bytes, kOffW2Hi = 2 * kW1Bytes,
                    kOffW2Lo = 2 * kW1Bytes + kW2Bytes, kOffVec = 2 * kW1Bytes + 2 * kW2Bytes;
 constexpr uint32_t kVecFloats = 3 * kN + 4;   // b2 | 0.505 w3 | 0.495 w3 | b3
-constexpr uint32_t kOffBar = kOffVec + kVecFloats * 4;
-constexpr uint32_t kOffFlag = kOffBar + 12 * 8;           // 12 mbarrier slots (10 used)
-constexpr uint32_t kSmemBytes = kOffFlag + 2 * kSlots * kRows;   // mask bits [parity][builder slot][row]
 // image = [W1hi | W1lo | W2hi | W2lo | vec] exactly as it sits in shared memory
-constexpr uint32_t kImageBytes = kOffBar;
+constexpr uint32_t kImageBytes = kOffVec + kVecFloats * 4;
+// the layer-1 operand tile: hi | lo, each kRows x kK1 halves as K-major core matrices
+constexpr uint32_t kALoOff = kRows * kK1 * 2;
+constexpr uint32_t kOffA = (kImageBytes + 127) & ~127u;
+constexpr uint32_t kOffBar = kOffA + 2 * kALoOff;
+constexpr uint32_t kOffFlag = kOffBar + 8 * 8;                  // 8 mbarrier slots (5 used)
+constexpr uint32_t kSmemBytes = kOffFlag + kSlots * kRows;     // mask bits [builder slot][row]
+static_assert(kSmemBytes <= 227 * 1024, "shared-memory budget of one CTA");
+// operand strides: one 8-wide K chunk of the A tile / of a 128-row weight matrix
+constexpr uint32_t kALbo = kRows * 16, kWLbo = kN * 16, kSbo = 128;
 
 // K-major no-swizzle core-matrix offset (in halves) of element (n, k) of an N x Kp operand
 __host__ __device__ inline uint32_t core_offset(int n, int k, int N) {
@@ -138,22 +86,9 @@ __host__ __device__ inline uint32_t core_offset(int n, int k, int N) {
 }
 
 // reference channel index (modules/cost_volume.py:698-723 order) of OUR layer-1 K position;
-// -2 = the bias position (constant one in A), -1 = padding.  The 21 pose measures (comb, r, t per
-// view) are NOT in K: they are constant per (frame, view), so their layer-1 contribution is a
-// per-frame bias vector (tc_frame_bias_kernel) added in the layer-1 epilogue.
+// -1 = padding.  The 21 pose measures (comb, r, t per view) are NOT in K: they are constant per
+// (frame, view), so their layer-1 contribution is a per-frame bias vector (tc_frame_bias_kernel).
 __host__ __device__ inline int ref_channel(int kk) {
-  if (kSplitView >= 0 && kk / kBlk == kSplitView) {
-    // the split view's block is two units of 12 K positions, unit h =
-    //   8 warped features (channels 8h..8h+7) | partial dot over those channels | three measures:
-    //   h = 0: mask, z', ray angle      h = 1: n_src (3)
-    // The dot appears twice (both partial sums meet the same W1 column; the MMA adds them).
-    const int k = kk / kBlk, j = kk - k * kBlk, h = j / (kBlk / 2), i = j - h * (kBlk / 2);
-    const int base = kC * (kViews + 1);
-    if (i < 8) return k * kC + 8 * h + i;
-    if (i == 8) return base + 2 * kViews + 1 + k;          // dot
-    if (h == 0) return i == 9 ? base + k : (i == 10 ? base + kViews + k : base + 3 * kViews + 1 + k);
-    return base + 4 * kViews + 4 + 3 * k + (i - 9);        // n_src
-  }
   if (kk < kViews * kBlk) {
     const int k = kk / kBlk, j = kk - k * kBlk;
     if (j < kC) return k * kC + j;                       // warped features
@@ -171,7 +106,6 @@ __host__ __device__ inline int ref_channel(int kk) {
   if (j < kC) return kViews * kC + j;                    // reference-frame features
   if (j == kC) return kC * (kViews + 1) + 2 * kViews;    // plane depth
   if (j < kC + 4) return kC * (kViews + 1) + 4 * kViews + 1 + (j - kC - 1);  // n_cur
-  if (kk == kBiasPos) return -2;                         // bias
   return -1;                                             // pad
 }
 // reference channels of the pose measures of view k: comb, r, t (:718-720)
@@ -193,7 +127,7 @@ tc_pack_kernel(srcv_mlp_weights w, uint8_t* __restrict__ image) {
     if (i < n1) {
       const int n = i / kK1, kk = i - n * kK1;
       const int f = ref_channel(kk);
-      const float v = kWScale * (f >= 0 ? w.w1[(size_t)n * kF + f] : (f == -2 ? w.b1[n] : 0.f));
+      const float v = kWScale * (f >= 0 ? w.w1[(size_t)n * kF + f] : 0.f);
       const __half h = __float2half_rn(v);
       w1hi[core_offset(n, kk, kN)] = h;
       w1lo[core_offset(n, kk, kN)] = __float2half_rn(v - __half2float(h));
@@ -228,18 +162,20 @@ tc_frame_bias_kernel(srcv_mlp_weights w, const ViewParams* __restrict__ views, f
     acc += (double)w.w1[(size_t)n * kF + pose_channel(1, k)] * (double)vp.rmeas;
     acc += (double)w.w1[(size_t)n * kF + pose_channel(2, k)] * (double)vp.tmeas;
   }
-  // + b1: the MMA issuer writes this vector, split into fp16 (hi, lo), into W1's bias row whenever its
-  // CTA moves on to another frame, so the whole layer-1 bias rides in the MMA (constant-one K position)
   pb[(size_t)b * kN + n] = (float)((double)kWScale * (acc + (double)w.b1[n]));
 }
 
-// 12 packed columns of one K block -> TMEM (hi and lo regions of the tile's A1 buffer)
-__device__ __forceinline__ void store_block(uint32_t a1_lane, uint32_t col, const uint32_t (&hi)[kBlkCols],
+// 12 packed columns of one K block -> the A tile in shared memory (hi and lo halves).  `a_row`
+// points at the row's first core-matrix line; column c (K 2c, 2c + 1) sits in K chunk c / 4, so a
+// block (12 columns, starting at a multiple of 4) is three 16-byte stores per half.
+__device__ __forceinline__ void store_block(uint8_t* a_row, uint32_t col, const uint32_t (&hi)[kBlkCols],
                                             const uint32_t (&lo)[kBlkCols]) {
-  st_x8(a1_lane + col, hi);
-  st_x4(a1_lane + col + 8, hi + 8);
-  st_x8(a1_lane + kA1LoOff + col, lo);
-  st_x4(a1_lane + kA1LoOff + col + 8, lo + 8);
+#pragma unroll
+  for (int i = 0; i < 3; ++i) {
+    uint8_t* p = a_row + ((col >> 2) + (uint32_t)i) * kALbo;
+    *reinterpret_cast<uint4*>(p) = uint4{hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]};
+    *reinterpret_cast<uint4*>(p + kALoOff) = uint4{lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]};
+  }
 }
 
 // What a worker thread keeps about the tile it builds the A operand for.
@@ -309,8 +245,7 @@ __device__ __forceinline__ unsigned view_block(const RowCtx& rc, const ViewParam
   }
   // features are sampled even for points behind the camera (only the dot is masked,
   // reference modules/cost_volume.py:590-623)
-  // blend and dot on packed pairs (FFMA2 / FMUL2: two IEEE fp32 operations per issue slot — the
-  // builders are issue-bound, not FMA-pipe-bound)
+  // blend and dot on (even, odd) channel pairs
   float2 v2[kC / 2];
   {
     const float4 *q0 = view4 + o00, *q1 = view4 + o01, *q2 = view4 + o10, *q3 = view4 + o11;
@@ -361,7 +296,7 @@ __device__ __forceinline__ unsigned view_block(const RowCtx& rc, const ViewParam
   return bits;
 }
 
-// The view-independent tail block: reference features | plane depth | n_cur | one | zeros
+// The view-independent tail block: reference features | plane depth | n_cur | zeros
 __device__ __forceinline__ void tail_block(const RowCtx& rc, uint32_t (&hi)[kBlkCols], uint32_t (&lo)[kBlkCols]) {
 #pragma unroll
   for (int j = 0; j < 4; ++j) {
@@ -370,165 +305,8 @@ __device__ __forceinline__ void tail_block(const RowCtx& rc, uint32_t (&hi)[kBlk
   }
   split_pack(rc.dval, rc.cx, hi[8], lo[8]);
   split_pack(rc.cy, rc.cz, hi[9], lo[9]);
-  hi[10] = 0x00003C00u; lo[10] = 0u;      // (1.0, 0): the bias position
-  hi[11] = 0u; lo[11] = 0u;
-}
-
-// ---- half-view unit: how view kSplitView is built ------------------------------------------------
-// A unit = one source view, channels 8h..8h+7: eight vector gathers, eight warped channels, the
-// partial dot over those channels and three of the view's six per-sample measures = 6 packed
-// columns.  The projection is done by both threads that share the view (~70 instructions each);
-// what moves off the critical slots is half of the gathers, the blend, the split and the stores.
-constexpr int kUnitCols = kBlkCols / 2;     // 6
-
-// what the conversion of a unit needs once its gathers are under way
-struct UnitCtx {
-  float w00, w01, w10, w11;   // bilinear weights (zeros-padding taps: 0)
-  float mk, e0, e1, e2;       // depth validity of the view; the unit's three measures
-};
-
-// project, set the footprint up and ISSUE the unit's eight gathers (f: [tap][chunk of the half])
-template <int TW, int HWC>
-__device__ __forceinline__ unsigned unit_issue(const RowCtx& rc, int k, int half, const float4* __restrict__ src4,
-                                               const ViewParams* __restrict__ views, int Wrt, int H, int HWrt,
-                                               const Centre& ctr, bool want_bits, UnitCtx& uc, float4 (&f)[4][2]) {
-  const int W = TW ? TW : Wrt, HW = HWC ? HWC : HWrt;
-  const ViewParams* vpp = views + (rc.b * kViews + k);
-  const float4* view4 = src4 + ((size_t)(rc.b * kViews + k) * 4 + 2 * half) * HW;
-  ViewRegs vr;
-  load_view(vpp, vr);
-  const float ax = fmaf(vr.hx[0], rc.dxc, fmaf(vr.hy[0], rc.dyc, vr.a0[0]));
-  const float ay = fmaf(vr.hx[1], rc.dxc, fmaf(vr.hy[1], rc.dyc, vr.a0[1]));
-  const float az = fmaf(vr.hx[2], rc.dxc, fmaf(vr.hy[2], rc.dyc, vr.a0[2]));
-  float px, py, zp;
-  project_point(rc.dval, ax, ay, az, vr.t[0], vr.t[1], vr.t[2], px, py, zp);
-  const float x0f = floorf(px), y0f = floorf(py);
-  const float fx = px - x0f, fy = py - y0f;
-  const bool inside = x0f >= -(float)ctr.nx && x0f <= (float)(W - 2 - ctr.nx) &&
-                      y0f >= -(float)ctr.ny && y0f <= (float)(H - 2 - ctr.ny);
-  const bool interior = __all_sync(0xffffffffu, inside);
-  const float gx = 1.0f - fx, gy = 1.0f - fy;
-  uc.w00 = gx * gy; uc.w01 = fx * gy; uc.w10 = gx * fy; uc.w11 = fx * fy;
-  int o00, o01, o10, o11;
-  if (interior) {
-    o00 = ((int)y0f + ctr.ny) * W + ((int)x0f + ctr.nx);
-    o01 = o00 + 1; o10 = o00 + W; o11 = o00 + W + 1;
-  } else {
-    // border patches, branch-free: clamped (in-range) addresses, zero weights for padding taps
-    Taps tp;
-    bilinear_taps(px, py, W, H, ctr, tp);
-    const int cxa = min(max(tp.x0, 0), W - 1), cxb = min(max(tp.x0 + 1, 0), W - 1);
-    const int cya = min(max(tp.y0, 0), H - 1) * W, cyb = min(max(tp.y0 + 1, 0), H - 1) * W;
-    o00 = cya + cxa; o01 = cya + cxb; o10 = cyb + cxa; o11 = cyb + cxb;
-    uc.w00 = (tp.valid & 1u) ? uc.w00 : 0.f; uc.w01 = (tp.valid & 2u) ? uc.w01 : 0.f;
-    uc.w10 = (tp.valid & 4u) ? uc.w10 : 0.f; uc.w11 = (tp.valid & 8u) ? uc.w11 : 0.f;
-  }
-  {
-    const float4 *q0 = view4 + o00, *q1 = view4 + o01, *q2 = view4 + o10, *q3 = view4 + o11;
 #pragma unroll
-    for (int j = 0; j < 2; ++j) {
-#ifdef SRCV_TC_ABL_NOGATHER   // ablation build (wrong results): how much of a tile is gather latency?
-      f[0][j] = f[1][j] = f[2][j] = f[3][j] = make_float4(uc.w00, uc.w01, (float)(o00 + o11), (float)(o01 + o10 + (int)(size_t)q0));
-      (void)q1; (void)q2; (void)q3;
-#else
-      f[0][j] = __ldg(q0 + (size_t)j * HW);
-      f[1][j] = __ldg(q1 + (size_t)j * HW);
-      f[2][j] = __ldg(q2 + (size_t)j * HW);
-      f[3][j] = __ldg(q3 + (size_t)j * HW);
-#endif
-    }
-  }
-  // the view's measures (independent of the gathers): mask, z', ray angle | n_src
-  const float mk = zp > 0.0f ? 1.0f : 0.0f;
-  const float sx0 = rc.X - vr.centre[0], sy0 = rc.Y - vr.centre[1], sz0 = rc.Z - vr.centre[2];
-  const float is = inv_norm(fmaf(sx0, sx0, fmaf(sy0, sy0, sz0 * sz0)), kEpsNorm);
-  const float sx = sx0 * is, sy = sy0 * is, sz = sz0 * is;
-  // cosine_similarity divides each operand by max(|.|, 1e-5) again (:683-688): both are unit vectors to
-  // an ulp here (or exactly zero, which stays zero), so the plain dot product is the same to ~1e-7
-  const float ang = fmaf(rc.cx, sx, fmaf(rc.cy, sy, rc.cz * sz));
-  uc.mk = mk;
-  uc.e0 = half ? sx : mk;
-  uc.e1 = half ? sy : zp;
-  uc.e2 = half ? sz : ang;
-  unsigned bits = 0;
-  if (want_bits) {
-    if (zp > 0.0f) bits |= 1u;
-    if (in_mask_bounds(px, py, W, H, ctr)) bits |= 2u;
-  }
-  return bits;
-}
-
-// bilinear blend, partial dot, (hi, lo) split and the unit's 6 + 6 packed columns -> TMEM
-__device__ __forceinline__ void unit_convert(const RowCtx& rc, int k, int half, const UnitCtx& uc,
-                                             const float4 (&f)[4][2], uint32_t a1_lane) {
-  const float2 p00 = make_float2(uc.w00, uc.w00), p01 = make_float2(uc.w01, uc.w01),
-               p10 = make_float2(uc.w10, uc.w10), p11 = make_float2(uc.w11, uc.w11);
-  float2 v2[4], d2 = make_float2(0.f, 0.f);
-#pragma unroll
-  for (int j = 0; j < 2; ++j) {
-    v2[2 * j] = fma2(p11, make_float2(f[3][j].x, f[3][j].y), fma2(p10, make_float2(f[2][j].x, f[2][j].y),
-                fma2(p01, make_float2(f[1][j].x, f[1][j].y), mul2(p00, make_float2(f[0][j].x, f[0][j].y)))));
-    v2[2 * j + 1] = fma2(p11, make_float2(f[3][j].z, f[3][j].w), fma2(p10, make_float2(f[2][j].z, f[2][j].w),
-                    fma2(p01, make_float2(f[1][j].z, f[1][j].w), mul2(p00, make_float2(f[0][j].z, f[0][j].w)))));
-    const float4 c = half ? rc.cur4[2 + j] : rc.cur4[j];
-    d2 = fma2(v2[2 * j], make_float2(c.x, c.y), d2);
-    d2 = fma2(v2[2 * j + 1], make_float2(c.z, c.w), d2);
-  }
-  uint32_t hi[kUnitCols], lo[kUnitCols];
-#pragma unroll
-  for (int i = 0; i < 4; ++i) split_pack(v2[i].x, v2[i].y, hi[i], lo[i]);
-  split_pack((d2.x + d2.y) * uc.mk, uc.e0, hi[4], lo[4]);
-  split_pack(uc.e1, uc.e2, hi[5], lo[5]);
-  const uint32_t col = (uint32_t)(kBlkCols * k + kUnitCols * half);
-  st_x4(a1_lane + col, hi);
-  st_x2(a1_lane + col + 4, hi + 4);
-  st_x4(a1_lane + kA1LoOff + col, lo);
-  st_x2(a1_lane + kA1LoOff + col + 4, lo + 4);
-}
-
-// Optional per-tile timeline of CTA 0 (experiment builds only, -DSRCV_TC_TIMELINE): one lane of
-// each role stamps %globaltimer-free SM clocks at its phase boundaries; read back with
-// srcv_debug_read_timeline.  Not compiled into the shipped library.
-#ifdef SRCV_TC_TIMELINE
-constexpr int kTlTiles = 48, kTlEvents = 16;
-__device__ long long g_timeline[kTlTiles * kTlEvents];
-#define SRCV_TL(it, ev)                                                                            \
-  do {                                                                                             \
-    if (blockIdx.x == 0 && lane == 0 && (warp & 3) == 0 && (it) < (unsigned)kTlTiles)                \
-      g_timeline[(it) * kTlEvents + (ev)] = clock64();                                             \
-  } while (0)
-#else
-#define SRCV_TL(it, ev) do { } while (0)
-#endif
-
-// issue D (+)= A_hi W_hi + A_hi W_lo + A_lo W_hi over the K steps [KS0, KS1) of 16, for the N
-// accumulator columns whose weight rows start at smem_hi / smem_lo (row n of a K chunk sits 16 n
-// bytes into it, so a column half is a start-address offset; the K-chunk stride stays kN * 16).
-// LAYER2: the operand sits where the layer-1 accumulator was — k-step ks reads the hi columns
-// 32 (ks / 2) + 8 (ks % 2) and the lo columns 16 further (see the layer-1 epilogue).
-#ifdef SRCV_TC_NO_SPLIT_HALVES   // experiment switch: whole-layer MMAs, epilogue and tensor pipe take turns
-constexpr bool kSplitHalves = false;
-#else
-constexpr bool kSplitHalves = true;
-#endif
-
-template <int N, int KS0, int KS1, bool LAYER2>
-__device__ __forceinline__ void issue_steps(uint32_t d, uint32_t a_base, uint32_t a_lo_off,
-                                            uint32_t smem_hi, uint32_t smem_lo) {
-  constexpr uint32_t idesc = idesc_f16_f32(kRows, N);
-  constexpr uint32_t kLbo = kN * 16, kSbo = 128, kStepBytes = 2 * kLbo;  // two 8-wide K chunks per MMA
-  // only the 14-bit start-address field changes from step to step
-  uint64_t bhi = smem_desc(smem_hi + KS0 * kStepBytes, kLbo, kSbo), blo = smem_desc(smem_lo + KS0 * kStepBytes, kLbo, kSbo);
-#pragma unroll 1
-  for (int ks = KS0; ks < KS1; ++ks) {
-    const uint32_t ahi = LAYER2 ? a_base + 32u * (uint32_t)(ks >> 1) + 8u * (uint32_t)(ks & 1)
-                                : a_base + 8u * (uint32_t)ks;
-    const uint32_t alo = ahi + a_lo_off;
-    mma_ts(d, ahi, bhi, idesc, ks > 0 ? 1u : 0u);
-    mma_ts(d, ahi, blo, idesc, 1u);
-    mma_ts(d, alo, bhi, idesc, 1u);
-    bhi += kStepBytes >> 4; blo += kStepBytes >> 4;
-  }
+  for (int j = 10; j < kBlkCols; ++j) hi[j] = lo[j] = 0u;
 }
 
 // tile id runs plane-chunk fastest, then pixel patch, then frame (32-bit: the launcher
@@ -592,6 +370,23 @@ __device__ __forceinline__ unsigned build_block(const RowCtx& rc, int blk, const
   return 0u;
 }
 
+// where the cost of tile row `row` goes: < 0 for rows outside the volume (integer part of make_row)
+struct RowOut {
+  long long out;
+  bool last_plane;
+};
+__device__ __forceinline__ RowOut row_out(unsigned id, int row, int W, int H, int HW, int D, const DivNd& nd,
+                                          unsigned tiles_x, unsigned tiles_xy) {
+  const unsigned r = nd.div(id), txy = r % tiles_xy;
+  const int d0 = (int)(id - r * nd.nd) * kTileD;
+  const int b = (int)(r / tiles_xy);
+  const int x0 = (int)(txy % tiles_x) * kTileW, y0 = (int)(txy / tiles_x) * kTileH;
+  const int rx = row & (kTileW - 1), ry = (row >> 4) & (kTileH - 1), dd = row >> 5;
+  const int d = d0 + dd;
+  const bool active = (x0 + rx < W) && (y0 + ry < H) && (d < D);
+  return RowOut{active ? ((long long)b * D + d) * HW + ((y0 + ry) * W + (x0 + rx)) : -1, d == D - 1};
+}
+
 template <bool PER_PIXEL, int TW, int TH>
 __global__ void __launch_bounds__(kThreads, 1)
 mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __restrict__ src4,
@@ -600,24 +395,18 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
               const float* __restrict__ frame_bias, float* __restrict__ cost, uint8_t* __restrict__ mask_out,
               unsigned num_tiles) {
   SRCV_DYNAMIC_SMEM_ALIGNED(uint8_t, smem, 1024);
-  __shared__ uint32_t s_tmem_base;
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  // Barriers of a BUFFER (a1_full, d2_free) exist once per A1 buffer and complete every second
-  // tile: their waiters can lag two tiles, which a single phase bit could not tell apart.
-  uint64_t* bar_a1_full = bars + 0;   // [2] builders -> MMA: A1 of a tile is in TMEM          (384 arrivals)
-  uint64_t* bar_d2_free = bars + 2;   // [2] epilogues done reading D2: the buffer is free     (128 arrivals)
-  // Layer 1 runs as two 64-column halves so that the epilogue of the first half overlaps the MMAs
-  // of the second, and layer 2 as two K halves so that it starts on the first half's operand while
-  // the epilogue still converts the second: the tensor pipe and the epilogue warps stop taking turns.
-  uint64_t* bar_mma1 = bars + 4;      // [2] layer-1 MMAs of a column half done: DA half holds D1 (commit)
-  uint64_t* bar_a2_full = bars + 6;   // [2] epilogues -> MMA: A2 half written over its D1 half  (128 arrivals)
-  uint64_t* bar_mma2 = bars + 8;      // layer-2 MMAs done: D2 ready, DA free                 (commit)
-  uint64_t* bar_img = bars + 9;       // weight image landed in shared memory (bulk copies)
+  // Consumer warpgroup c takes the tiles it = c, c + 2, ...; each barrier below exists once per
+  // consumer, so that a waiter never sees a phase of the other warpgroup's tile.
+  uint64_t* bar_a1_full = bars + 0;   // [2] builders -> consumer c: the A tile is written   (256 arrivals)
+  uint64_t* bar_a1_free = bars + 2;   // [2] consumer c -> builders: its layer-1 MMAs are done (128 arrivals)
+  uint64_t* bar_img = bars + 4;       // weight image landed in shared memory (bulk copies)
   uint8_t* sflag = smem + kOffFlag;
+  uint8_t* sa = smem + kOffA;
   const float* svec = reinterpret_cast<const float*>(smem + kOffVec);
 
   // The warp index goes through a shuffle broadcast so that ptxas knows the role branches are
-  // warp-uniform and keeps the global-memory descriptors in uniform registers.
+  // warp-uniform.
   const int tid = threadIdx.x, warp = __shfl_sync(0xffffffffu, tid >> 5, 0), lane = tid & 31;
   const int W = TW ? TW : s.W, H = TH ? TH : s.H, HW = W * H, D = s.D;
   constexpr int HWC = TW * TH;
@@ -628,24 +417,16 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
   // ---- one-time setup ----------------------------------------------------------------
   if (tid == 0) {
     mbar_init(bar_img, 1);
-    mbar_init(bar_a1_full, kBuilders);
-    mbar_init(bar_a1_full + 1, kBuilders);
-    mbar_init(bar_d2_free, kEpis);
-    mbar_init(bar_d2_free + 1, kEpis);
-    mbar_init(bar_mma1, 1);
-    mbar_init(bar_mma1 + 1, 1);
-    mbar_init(bar_a2_full, kEpis);
-    mbar_init(bar_a2_full + 1, kEpis);
-    mbar_init(bar_mma2, 1);
+    for (int c = 0; c < kConsumers; ++c) {
+      mbar_init(bar_a1_full + c, kBuilders);
+      mbar_init(bar_a1_free + c, 128);
+    }
     mbar_fence_init();
   }
-  if (warp == kMmaWarp) tmem_alloc(&s_tmem_base, kTmemCols);
-  fence_before_sync();
   __syncthreads();
-  fence_after_sync();
-  // The 170 KB weight image (fp16 core matrices + biases) is pulled in by the bulk-copy
-  // (TMA) engine straight into shared memory — written by the async proxy, which is also
-  // the proxy the tensor core reads it through — while the threads finish their setup.
+  // The weight image (fp16 core matrices + biases) is pulled in by the bulk-copy (TMA) engine
+  // straight into shared memory — written by the async proxy, which is also the proxy the tensor
+  // core reads it through — while the threads finish their setup.
   if (tid == 0) {
     mbar_expect_tx(bar_img, kImageBytes);
     constexpr uint32_t kPiece = 32768;
@@ -653,272 +434,145 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
       bulk_g2s(smem + off, image + off, (kImageBytes - off < kPiece) ? (kImageBytes - off) : kPiece, bar_img);
   }
   mbar_wait(bar_img, 0);
-  const uint32_t tmem_base = s_tmem_base;
-  const uint32_t lane_base = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-  // Work split: CTA c takes tiles c, c + grid, c + 2 grid, ... of the plane-fastest tile
-  // order, i.e. at any moment the 148 CTAs sweep ~2 neighbouring pixel blocks x 64 planes of
-  // ONE frame, whose source features (39 MB) stay L2-resident, and every CTA sees the same mix
-  // of interior and border patches.
-#ifdef SRCV_TC_CONTIG
-  // experiment switch: one contiguous tile range per CTA (consecutive plane chunks of a patch)
-  const unsigned t_lo = (unsigned)(((unsigned long long)num_tiles * blockIdx.x) / gridDim.x);
-  const unsigned t_hi = (unsigned)(((unsigned long long)num_tiles * (blockIdx.x + 1)) / gridDim.x);
-  const unsigned n_local = t_hi - t_lo;
-  auto tile_id = [&](unsigned j) { return t_lo + j; };
-#else
+  // Work split: CTA c takes tiles c, c + grid, c + 2 grid, ... of the plane-fastest tile order, i.e.
+  // at any moment the CTAs sweep a few neighbouring pixel blocks x all planes of ONE frame, whose
+  // source features stay L2-resident, and every CTA sees the same mix of interior and border patches.
   const unsigned n_local = (num_tiles - blockIdx.x + gridDim.x - 1) / gridDim.x;
   auto tile_id = [&](unsigned j) { return blockIdx.x + j * gridDim.x; };
-#endif
 
   if (warp < kBuildWarps) {
     // =============================== builders ============================================
-    // Twelve warps: three threads per row (slot = warp / 4): two whole source views each, then half of
-    // view kSplitView (slots 0, 1) or the tail (slot 2).  With
-    // two A1 buffers they run up to a whole tile ahead of the tensor pipe: buffer t & 1 is free
-    // again once the layer-2 epilogue of tile t - 2 has read its accumulator out of it.
-    if (kSetmaxnreg && kRegsBuild > kRegsLaunch) reg_inc<kRegsBuild>();
-    const int row = (warp & 3) * 32 + lane, slot = warp >> 2;
+    // Four threads per row (slot = warp / 2): views 2 slot, 2 slot + 1; slot 3 builds view 6 and the
+    // view-independent tail.  The first block of tile it is built before the wait for the operand
+    // tile, so its gathers overlap the layer-1 MMAs of tile it - 1.
+    reg_dec<kRegsBuild>();
+    const int row = (warp & 1) * 32 + lane, slot = warp >> 1;
     const Centre ctr(W, H);
-    // slot 0: views 0, 1 + the first half of view kSplitView; slot 1: views 3, 4 + its second half;
-    // slot 2: views 5, 6 + the tail
-    const int blk_first = kSlots == 4 ? 2 * slot : ((slot < 2) ? 3 * slot : 5);
+    const int blk_first = 2 * slot;
     const bool masks = mask_out != nullptr;
+    uint8_t* a_row = sa + (uint32_t)(row >> 3) * kSbo + (uint32_t)(row & 7) * 16u;
     RowCtx rc;
     uint32_t hi[kBlkCols], lo[kBlkCols];
     for (unsigned it = 0; it < n_local; ++it) {
-      const uint32_t buf = it & 1u, use = it >> 1;       // use-th tile of this buffer
-      SRCV_TL(it, 0);
       make_row<PER_PIXEL>(tile_id(it), row, W, H, HW, D, nd, tiles_x, tiles_xy, ctr, cur4g, frames, planes, rc);
       const bool wb = masks && rc.last_plane;
-      const uint32_t a1_lane = lane_base + kColA1 + buf * kA1Stride;
       unsigned bits = build_block<TW, HWC>(rc, blk_first, src4, views, W, H, HW, ctr, wb, hi, lo);
-      SRCV_TL(it, 1);
-      if (use > 0) {
-        mbar_wait(bar_d2_free + buf, (use - 1) & 1u);    // tile it - 2 is completely out of this buffer
-        fence_after_sync();
-      }
-      SRCV_TL(it, 2);
-      store_block(a1_lane, (uint32_t)(kBlkCols * blk_first), hi, lo);
-      bits |= build_block<TW, HWC>(rc, blk_first + 1, src4, views, W, H, HW, ctr, wb, hi, lo);   // slot 3 of 4: the tail
-      store_block(a1_lane, (uint32_t)(kBlkCols * (blk_first + 1)), hi, lo);
-      if (kSlots == 4) {
-        // two blocks per thread: done
-      } else if (slot < 2) {
-        float4 f[4][2];
-        UnitCtx uc;
-        bits |= unit_issue<TW, HWC>(rc, kSplitView, slot, src4, views, W, H, HW, ctr, wb, uc, f);
-        unit_convert(rc, kSplitView, slot, uc, f, a1_lane);
-      } else {
-        tail_block(rc, hi, lo);
-        store_block(a1_lane, (uint32_t)(kBlkCols * kViews), hi, lo);
-      }
-      // Mask bits of this tile live with its buffer: the epilogue warp reads them before its
-      // bar_d2_free arrival for this tile, and the next store into the slot (tile it + 2) follows
-      // this thread's wait on exactly that barrier phase.
-      if (wb) sflag[(buf * kSlots + slot) * kRows + row] = (uint8_t)bits;
-      wait_st();
-      fence_before_sync();
-      mbar_arrive(bar_a1_full + buf);
-      SRCV_TL(it, 3);
-    }
-  } else if (warp < kBuildWarps + kEpiWarps) {
-    // =============================== epilogues ===========================================
-    // Four warps, one thread per row.  Layer-1 epilogue: per-frame pose bias, LeakyReLU, (hi, lo)
-    // split, layer-2 operand written IN PLACE over the accumulator, 32 columns at a time (a
-    // chunk's 32 fp32 columns become its 16 hi + 16 lo operand columns).  Layer-2 epilogue: bias,
-    // LeakyReLU and the 128 -> 1 layer as one dot product per row — no cross-thread reduction.
-    if (kSetmaxnreg) reg_inc<kRegsEpi>();
-    const int row = (warp & 3) * 32 + lane;
-    const bool masks = mask_out != nullptr;
-    for (unsigned it = 0; it < n_local; ++it) {
-      const uint32_t par = it & 1u, buf = it & 1u;
-      // where this row's cost goes (integer part of make_row)
-      long long out;
-      bool last_plane;
-      int b;
-      {
-        const unsigned id = tile_id(it);
-        const unsigned r = nd.div(id), txy = r % tiles_xy;
-        const int d0 = (int)(id - r * nd.nd) * kTileD;
-        b = (int)(r / tiles_xy);
-        const int x0 = (int)(txy % tiles_x) * kTileW, y0 = (int)(txy / tiles_x) * kTileH;
-        const int rx = row & (kTileW - 1), ry = (row >> 4) & (kTileH - 1), dd = row >> 5;
-        const int d = d0 + dd;
-        const bool active = (x0 + rx < W) && (y0 + ry < H) && (d < D);
-        out = active ? ((long long)b * D + d) * HW + ((y0 + ry) * W + (x0 + rx)) : -1;
-        last_plane = (d == D - 1);
-      }
-      // kEpiStep columns per step (64: two TMEM loads in flight per wait, twice the independent
-      // work per dependent chain; 32 where the register budget of this group is 96)
-#pragma unroll 1
-      for (int c = 0; c < kN; c += kEpiStep) {
-        if ((c & 63) == 0 && (kSplitHalves || c == 0)) {
-          mbar_wait(bar_mma1 + (c >> 6), par);   // this column half of D1 is complete
-          fence_after_sync();
-          SRCV_TL(it, c ? 14 : 4);
-        }
-        uint32_t r[kEpiStep];
-#pragma unroll
-        for (int h = 0; h < kEpiStep / 32; ++h) ld_x32(lane_base + kColDA + c + 32 * h, r + 32 * h);
-        wait_ld();
-#pragma unroll
-        for (int h = 0; h < kEpiStep / 32; ++h) {
-          uint32_t ehi[16], elo[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            // LeakyReLU = max(x, 0.01 x), the multiply as one packed FMUL2 per column pair (the
-            // bias, incl. the frame's pose measures, came out of the MMA)
-            const float2 x = make_float2(__uint_as_float(r[32 * h + 2 * j]), __uint_as_float(r[32 * h + 2 * j + 1]));
-            const float2 m = mul2(x, make_float2(kLeaky, kLeaky));
-            split_pack(fmaxf(x.x, m.x), fmaxf(x.y, m.y), ehi[j], elo[j]);
-          }
-          st_x16(lane_base + kColDA + c + 32 * h, ehi);
-          st_x16(lane_base + kColDA + c + 32 * h + 16, elo);
-        }
-        if (((c + kEpiStep) & 63) == 0 && (kSplitHalves || c + kEpiStep == kN)) {
-          wait_st();
-          fence_before_sync();
-          mbar_arrive(bar_a2_full + (c >> 6));   // k-steps 4 (c / 64) .. + 3 of the layer-2 operand
-          SRCV_TL(it, (c >> 6) ? 5 : 13);
-        }
-      }
-      // mask bits of the builders: visible since the bar_mma1 waits above (a1_full -> MMA -> commit)
-      unsigned tile_bits = 0;
-      if (masks && last_plane) {
-        const uint8_t* fl = sflag + buf * kSlots * kRows + row;
-#pragma unroll
-        for (int q = 0; q < kSlots; ++q) tile_bits |= fl[q * kRows];
-      }
-      // ---- layer-2 epilogue: the accumulator sits in the first 128 columns of this tile's A1 buffer
-      mbar_wait(bar_mma2, par);
-      fence_after_sync();
-      SRCV_TL(it, 6);
-      const uint32_t d2_lane = lane_base + kColA1 + buf * kA1Stride;
-      float2 acc2 = make_float2(0.f, 0.f);     // even / odd columns, as packed FFMA2 chains
-#pragma unroll 1
-      for (int c = 0; c < kN; c += kEpiStep) {
-        uint32_t r[kEpiStep];
-#pragma unroll
-        for (int h = 0; h < kEpiStep / 32; ++h) ld_x32(d2_lane + c + 32 * h, r + 32 * h);
-        wait_ld();
-        if (c == kN - kEpiStep) {
-          fence_before_sync();
-          mbar_arrive(bar_d2_free + buf);   // the buffer is free: the builders may write tile it + 2 into it
-          SRCV_TL(it, 7);
-        }
-#pragma unroll
-        for (int j = 0; j < kEpiStep; j += 4) {
-          const float4 bb = *reinterpret_cast<const float4*>(svec + c + j);
-          const float4 wa = *reinterpret_cast<const float4*>(svec + kN + c + j);
-          const float4 wn = *reinterpret_cast<const float4*>(svec + 2 * kN + c + j);
-          const float2 us = make_float2(kUnscale2, kUnscale2);
-          const float2 h01 = fma2(make_float2(__uint_as_float(r[j + 0]), __uint_as_float(r[j + 1])), us, make_float2(bb.x, bb.y));
-          const float2 h23 = fma2(make_float2(__uint_as_float(r[j + 2]), __uint_as_float(r[j + 3])), us, make_float2(bb.z, bb.w));
-          acc2 = fma2(make_float2(wn.x, wn.y), make_float2(fabsf(h01.x), fabsf(h01.y)), fma2(make_float2(wa.x, wa.y), h01, acc2));
-          acc2 = fma2(make_float2(wn.z, wn.w), make_float2(fabsf(h23.x), fabsf(h23.y)), fma2(make_float2(wa.z, wa.w), h23, acc2));
-        }
-      }
-      if (out >= 0) {
-        cost[out] = (acc2.x + acc2.y) + svec[3 * kN];
-        if (masks && last_plane) {
-          // overall mask of the LAST plane (reference :625-637): any view in front AND any view
-          // inside the 2-pixel border, independently
-          mask_out[(size_t)b * HW + (out - ((long long)b * D + (D - 1)) * HW)] = (tile_bits == 3u) ? 1 : 0;
-        }
-      }
-      SRCV_TL(it, 8);
+      if (it > 0) mbar_wait(bar_a1_free + ((it - 1) & 1u), ((it - 1) >> 1) & 1u);   // tile it - 1 is out of it
+      store_block(a_row, (uint32_t)(kBlkCols * blk_first), hi, lo);
+      bits |= build_block<TW, HWC>(rc, blk_first + 1, src4, views, W, H, HW, ctr, wb, hi, lo);
+      store_block(a_row, (uint32_t)(kBlkCols * (blk_first + 1)), hi, lo);
+      // the consumer of tile it reads the mask bits before it frees the operand tile, and the next
+      // store into this slot follows this thread's wait on exactly that arrival
+      if (wb) sflag[slot * kRows + row] = (uint8_t)bits;
+      fence_proxy_async_smem();                    // generic-proxy stores -> visible to wgmma
+      mbar_arrive(bar_a1_full + (it & 1u));
     }
   } else {
-    if (kSetmaxnreg) reg_dec<kRegsMma>();
-    if (warp == kMmaWarp) {
-      // =============================== MMA issuer ==========================================
-      const uint32_t sbase = smem_u32(smem);
-      __half* w1hi = reinterpret_cast<__half*>(smem + kOffW1Hi);
-      __half* w1lo = reinterpret_cast<__half*>(smem + kOffW1Lo);
-      int bias_frame = -1;
-      for (unsigned it = 0; it < n_local; ++it) {
-        const uint32_t par = it & 1u, buf = it & 1u, use = it >> 1;
-        const uint32_t a1 = tmem_base + kColA1 + buf * kA1Stride;
-        // The layer-1 bias of the tile's frame (b1 + its pose measures) is W1's row at the constant-one
-        // K position: rewritten (fp16 hi, lo) when the CTA's tiles move on to another frame.  Its
-        // readers — the layer-1 MMAs of earlier tiles — completed before this warp issued the
-        // previous tile's last layer-2 MMAs (bar_mma1 -> epilogue -> bar_a2_full -> here).
-        const int fb = (int)(nd.div(tile_id(it)) / tiles_xy);
-        if (fb != bias_frame) {
-          bias_frame = fb;
+    // =============================== consumers ===========================================
+    reg_inc<kRegsCons>();
+    const int c = (warp - kBuildWarps) >> 2, wl = (warp - kBuildWarps) & 3;
+    const int g = lane >> 2, q = lane & 3;
+    const int r0 = 16 * wl + g, r1 = r0 + 8;       // the two tile rows of this thread's fragments
+    const bool masks = mask_out != nullptr;
+    const uint32_t sbase = smem_u32(smem);
+    for (unsigned k = 0, it = (unsigned)c; it < n_local; ++k, it += kConsumers) {
+      const unsigned id = tile_id(it);
+      const int b = (int)(nd.div(id) / tiles_xy);
+      const RowOut o0 = row_out(id, r0, W, H, HW, D, nd, tiles_x, tiles_xy);
+      const RowOut o1 = row_out(id, r1, W, H, HW, D, nd, tiles_x, tiles_xy);
+      mbar_wait(bar_a1_full + c, k & 1u);
+      unsigned bits0 = 0, bits1 = 0;
+      if (masks && q == 0) {
 #pragma unroll
-          for (int i = 0; i < kN / 32; ++i) {
-            const int n = lane + 32 * i;
-            const float v = __ldg(frame_bias + (size_t)fb * kN + n);
-            const __half h = __float2half_rn(v);
-            w1hi[core_offset(n, kBiasPos, kN)] = h;
-            w1lo[core_offset(n, kBiasPos, kN)] = __float2half_rn(v - __half2float(h));
-          }
-          fence_proxy_async_smem();                // generic-proxy stores -> visible to the tensor core
-          __syncwarp();
+        for (int sl = 0; sl < kSlots; ++sl) {
+          if (o0.last_plane) bits0 |= sflag[sl * kRows + r0];
+          if (o1.last_plane) bits1 |= sflag[sl * kRows + r1];
         }
-        mbar_wait(bar_a1_full + buf, use & 1u);   // A1 of this tile is in TMEM
-        fence_after_sync();
-        SRCV_TL(it, 9);
-        // DA is free: the layer-2 MMAs of the previous tile (its last readers) were issued before
-        // these and the tensor pipe executes this thread's MMAs in order.
-        if (kSplitHalves) {
-          if (elect_one()) {
-            issue_steps<kN / 2, 0, kK1 / 16, false>(tmem_base + kColDA, a1, kA1LoOff, sbase + kOffW1Hi, sbase + kOffW1Lo);
-            mma_commit(bar_mma1);
-            issue_steps<kN / 2, 0, kK1 / 16, false>(tmem_base + kColDA + kN / 2, a1, kA1LoOff,
-                                                    sbase + kOffW1Hi + (kN / 2) * 16, sbase + kOffW1Lo + (kN / 2) * 16);
-            mma_commit(bar_mma1 + 1);
-          }
-          __syncwarp();
-          SRCV_TL(it, 10);
-          mbar_wait(bar_a2_full, par);             // first half of A2 written over D1
-          fence_after_sync();
-          SRCV_TL(it, 11);
-          // D2 goes into this tile's own A1 buffer: its layer-1 MMAs (just above, same in-order
-          // pipe) are the last readers, and the builders do not touch it before bar_d2_free.
-          if (elect_one())
-            issue_steps<kN, 0, kK2 / 32, true>(a1, tmem_base + kColDA, 16u, sbase + kOffW2Hi, sbase + kOffW2Lo);
-          __syncwarp();
-          mbar_wait(bar_a2_full + 1, par);         // second half
-          fence_after_sync();
-          SRCV_TL(it, 15);
-          if (elect_one()) {
-            issue_steps<kN, kK2 / 32, kK2 / 16, true>(a1, tmem_base + kColDA, 16u, sbase + kOffW2Hi, sbase + kOffW2Lo);
-            mma_commit(bar_mma2);
-          }
-        } else {
-          if (elect_one()) {
-            issue_steps<kN, 0, kK1 / 16, false>(tmem_base + kColDA, a1, kA1LoOff, sbase + kOffW1Hi, sbase + kOffW1Lo);
-            mma_commit(bar_mma1);
-          }
-          __syncwarp();
-          SRCV_TL(it, 10);
-          mbar_wait(bar_a2_full + 1, par);         // A2 written over D1
-          fence_after_sync();
-          SRCV_TL(it, 11);
-          if (elect_one()) {
-            issue_steps<kN, 0, kK2 / 16, true>(a1, tmem_base + kColDA, 16u, sbase + kOffW2Hi, sbase + kOffW2Lo);
-            mma_commit(bar_mma2);
+      }
+      // ---- layer 1: D1 = 16 (W1 x) over 12 k-steps, three products each
+      float d1[64];
+      wgmma_fence();
+#pragma unroll 1
+      for (int ks = 0; ks < kK1 / 16; ++ks) {
+        const uint32_t ahi = sbase + kOffA + (uint32_t)ks * 2 * kALbo;
+        const uint32_t bhi = sbase + kOffW1Hi + (uint32_t)ks * 2 * kWLbo, blo = bhi + kW1Bytes;
+        wgmma_ss_n128(d1, smem_desc(ahi, kALbo, kSbo), smem_desc(bhi, kWLbo, kSbo), ks > 0 ? 1u : 0u);
+        wgmma_ss_n128(d1, smem_desc(ahi, kALbo, kSbo), smem_desc(blo, kWLbo, kSbo), 1u);
+        wgmma_ss_n128(d1, smem_desc(ahi + kALoOff, kALbo, kSbo), smem_desc(bhi, kWLbo, kSbo), 1u);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(d1);
+      mbar_arrive(bar_a1_free + c);                // the builders may write tile it + 1
+      // ---- layer-1 epilogue: + frame bias, LeakyReLU, (hi, lo) split into the layer-2 A fragments
+      uint32_t a2hi[kK2 / 16][4], a2lo[kK2 / 16][4];
+      const float* pb = frame_bias + (size_t)b * kN + 2 * q;
+#pragma unroll
+      for (int j = 0; j < kN / 8; ++j) {
+        const float2 bb = __ldg(reinterpret_cast<const float2*>(pb + 8 * j));
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const float x0 = leaky(d1[4 * j + 2 * h] + bb.x), x1 = leaky(d1[4 * j + 2 * h + 1] + bb.y);
+          split_pack(x0, x1, a2hi[j >> 1][2 * (j & 1) + h], a2lo[j >> 1][2 * (j & 1) + h]);
+        }
+      }
+      // ---- layer 2 in two 64-column halves, each followed by its share of the 128 -> 1 layer
+      float acc0 = 0.f, acc1 = 0.f;                // rows r0, r1
+#pragma unroll 1
+      for (int nh = 0; nh < 2; ++nh) {
+        float d2[32];
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < kK2 / 16; ++ks) {
+          const uint32_t bhi = sbase + kOffW2Hi + (uint32_t)nh * (kN / 2) * 16 + (uint32_t)ks * 2 * kWLbo;
+          const uint32_t blo = bhi + kW2Bytes;
+          wgmma_rs_n64(d2, a2hi[ks], smem_desc(bhi, kWLbo, kSbo), ks > 0 ? 1u : 0u);
+          wgmma_rs_n64(d2, a2hi[ks], smem_desc(blo, kWLbo, kSbo), 1u);
+          wgmma_rs_n64(d2, a2lo[ks], smem_desc(bhi, kWLbo, kSbo), 1u);
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        fence_regs(d2);
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          const int n = nh * (kN / 2) + 8 * j + 2 * q;
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int nn = n + (e & 1);
+            const float hv = fmaf(d2[4 * j + e], kUnscale2, svec[nn]);
+            const float t = fmaf(svec[2 * kN + nn], fabsf(hv), svec[kN + nn] * hv);
+            if (e < 2) acc0 += t; else acc1 += t;
           }
         }
-        __syncwarp();
-        SRCV_TL(it, 12);
+      }
+      // the four threads of a quad hold the four column subsets of the same two rows
+      acc0 += __shfl_xor_sync(0xffffffffu, acc0, 1);
+      acc1 += __shfl_xor_sync(0xffffffffu, acc1, 1);
+      acc0 += __shfl_xor_sync(0xffffffffu, acc0, 2);
+      acc1 += __shfl_xor_sync(0xffffffffu, acc1, 2);
+      if (q == 0) {
+        const float b3 = svec[3 * kN];
+        // overall mask of the LAST plane (reference :625-637): any view in front AND any view
+        // inside the 2-pixel border, independently
+        if (o0.out >= 0) {
+          cost[o0.out] = acc0 + b3;
+          if (masks && o0.last_plane)
+            mask_out[(size_t)b * HW + (o0.out - ((long long)b * D + (D - 1)) * HW)] = (bits0 == 3u) ? 1 : 0;
+        }
+        if (o1.out >= 0) {
+          cost[o1.out] = acc1 + b3;
+          if (masks && o1.last_plane)
+            mask_out[(size_t)b * HW + (o1.out - ((long long)b * D + (D - 1)) * HW)] = (bits1 == 3u) ? 1 : 0;
+        }
       }
     }
-  }
-  // ---- teardown ---------------------------------------------------------------------------
-  fence_before_sync();
-  __syncthreads();
-  if (warp == kMmaWarp) {
-    fence_after_sync();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
 // ------------------------------------------------------------------------------------------
-// self-test: D[128,128] = A[128,Kp] W[128,Kp]^T through the same TMEM / descriptor / barrier
-// machinery (A split and written to TMEM by the row threads, W packed to core matrices).
+// self-test: D[128,128] = A[128,Kp] W[128,Kp]^T through the same descriptors and (hi, lo) split as
+// layer 1 of the sweep (A split and written to shared memory by the threads, W packed to core
+// matrices), one 64-row half after the other.
 // ------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
 tc_selftest_pack(const float* __restrict__ Wm, int Kp, __half* __restrict__ hi, __half* __restrict__ lo) {
@@ -931,69 +585,48 @@ tc_selftest_pack(const float* __restrict__ Wm, int Kp, __half* __restrict__ hi, 
   }
 }
 
-__global__ void __launch_bounds__(160, 1)
+__global__ void __launch_bounds__(128, 1)
 tc_selftest_kernel(const float* __restrict__ A, const __half* __restrict__ whi,
                    const __half* __restrict__ wlo, int Kp, float* __restrict__ Dout) {
   SRCV_DYNAMIC_SMEM_ALIGNED(uint8_t, smem, 1024);
-  __shared__ uint32_t s_tmem_base;
-  __shared__ uint64_t bar_a, bar_d;
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const uint32_t wbytes = (uint32_t)kN * Kp * 2;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31, g = lane >> 2, q = lane & 3;
+  const uint32_t wbytes = (uint32_t)kN * Kp * 2, abytes = (uint32_t)kRows * Kp * 2;
+  uint8_t* sa = smem + 2 * wbytes;
   for (uint32_t i = tid; i < wbytes / 16; i += blockDim.x) {
     reinterpret_cast<uint4*>(smem)[i] = __ldg(reinterpret_cast<const uint4*>(whi) + i);
     reinterpret_cast<uint4*>(smem + wbytes)[i] = __ldg(reinterpret_cast<const uint4*>(wlo) + i);
   }
-  if (tid == 0) { mbar_init(&bar_a, 128); mbar_init(&bar_d, 1); mbar_fence_init(); }
-  if (warp == 4) tmem_alloc(&s_tmem_base, kTmemCols);
-  fence_proxy_async_smem();
-  fence_before_sync();
-  __syncthreads();
-  fence_after_sync();
-  const uint32_t tmem_base = s_tmem_base;
-  const uint32_t lane_base = tmem_base + ((uint32_t)((warp & 3) * 32) << 16);
-  const uint32_t col_lo = Kp / 2, col_d = 256;
-  if (warp < 4) {
-    const float* a = A + (size_t)tid * Kp;
-    for (int c = 0; c < Kp / 2; c += 8) {
-      uint32_t hi[8], lo[8];
+  const uint32_t sb = smem_u32(smem), lbo_w = kN * 16, lbo_a = kRows * 16;
+  for (int mh = 0; mh < 2; ++mh) {
+    for (int i = tid; i < kRows * Kp / 2; i += blockDim.x) {
+      const int r = i / (Kp / 2), cc = i - r * (Kp / 2);
+      const float* a = A + (size_t)(kRows * mh + r) * Kp + 2 * cc;
+      uint32_t h, l;
+      split_pack(a[0], a[1], h, l);
+      const uint32_t off = 2 * core_offset(r, 2 * cc, kRows);
+      *reinterpret_cast<uint32_t*>(sa + off) = h;
+      *reinterpret_cast<uint32_t*>(sa + abytes + off) = l;
+    }
+    fence_proxy_async_smem();
+    __syncthreads();
+    float d[64];
+    wgmma_fence();
+    for (int ks = 0; ks < Kp / 16; ++ks) {
+      const uint32_t ahi = sb + 2 * wbytes + ks * 2 * lbo_a, bhi = sb + ks * 2 * lbo_w;
+      wgmma_ss_n128(d, smem_desc(ahi, lbo_a, kSbo), smem_desc(bhi, lbo_w, kSbo), ks > 0 ? 1u : 0u);
+      wgmma_ss_n128(d, smem_desc(ahi, lbo_a, kSbo), smem_desc(bhi + wbytes, lbo_w, kSbo), 1u);
+      wgmma_ss_n128(d, smem_desc(ahi + abytes, lbo_a, kSbo), smem_desc(bhi, lbo_w, kSbo), 1u);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(d);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) split_pack(a[2 * (c + j)], a[2 * (c + j) + 1], hi[j], lo[j]);
-      st_x8(lane_base + c, hi);
-      st_x8(lane_base + col_lo + c, lo);
-    }
-    wait_st();
-    fence_before_sync();
-    mbar_arrive(&bar_a);
-    mbar_wait(&bar_d, 0);
-    fence_after_sync();
-    for (int c0 = 0; c0 < kN; c0 += 32) {
-      uint32_t r[32];
-      ld_x32(lane_base + col_d + c0, r);
-      wait_ld();
+    for (int j = 0; j < kN / 8; ++j)
 #pragma unroll
-      for (int j = 0; j < 32; ++j) Dout[(size_t)tid * kN + c0 + j] = __uint_as_float(r[j]);
-    }
-  } else {
-    mbar_wait(&bar_a, 0);
-    fence_after_sync();
-    if (lane == 0) {
-      constexpr uint32_t idesc = idesc_f16_f32(kRows, kN);
-      constexpr uint32_t kLbo = kN * 16, kSbo = 128;
-      const uint32_t sb = smem_u32(smem);
-      for (int ks = 0; ks < Kp / 16; ++ks) {
-        const uint64_t bhi = smem_desc(sb + ks * 2 * kLbo, kLbo, kSbo);
-        const uint64_t blo = smem_desc(sb + wbytes + ks * 2 * kLbo, kLbo, kSbo);
-        mma_ts(tmem_base + col_d, tmem_base + ks * 8, bhi, idesc, ks > 0 ? 1u : 0u);
-        mma_ts(tmem_base + col_d, tmem_base + ks * 8, blo, idesc, 1u);
-        mma_ts(tmem_base + col_d, tmem_base + col_lo + ks * 8, bhi, idesc, 1u);
-      }
-      mma_commit(&bar_d);
-    }
-    __syncwarp();
+      for (int e = 0; e < 4; ++e)
+        Dout[(size_t)(kRows * mh + 16 * warp + g + 8 * (e >> 1)) * kN + 8 * j + 2 * q + (e & 1)] = d[4 * j + e];
+    __syncthreads();                               // every MMA has read the A tile before it is rewritten
   }
-  fence_before_sync();
-  __syncthreads();
-  if (warp == 4) { fence_after_sync(); tmem_dealloc(tmem_base, kTmemCols); }
 }
 
 }  // namespace
@@ -1004,7 +637,7 @@ bool mlp_tc_supported(const srcv_shape& s, const srcv_mlp_weights& w) {
 }
 
 static size_t image_bytes_aligned() { return (kImageBytes + 255) & ~(size_t)255; }
-// workspace tail of the tensor-core variant: [weight image | per-frame pose bias (B x 128 floats)]
+// workspace tail of the tensor-core variant: [weight image | per-frame layer-1 bias (B x 128 floats)]
 size_t mlp_tc_extra_bytes(const srcv_shape& s) { return image_bytes_aligned() + (((size_t)s.B * kN * 4 + 255) & ~(size_t)255); }
 size_t mlp_tc_image_bytes() { return kImageBytes; }
 
@@ -1025,11 +658,11 @@ cudaError_t launch_mlp_tc(const srcv_shape& s, const float* cur, const Workspace
     if (err != cudaSuccess) return err;
     image = reinterpret_cast<const uint8_t*>(ws.extra);
   }
-  // the 21 pose measures enter layer 1 as a per-frame bias (views were written by the prep pass)
+  // b1 and the 21 pose measures enter layer 1 as a per-frame bias (views were written by the prep pass)
   float* frame_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws.extra) + image_bytes_aligned());
   SRCV_LAUNCH(tc_frame_bias_kernel, s.B, kN, 0, stream, w, ws.views, frame_bias);
   note_launch();
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 1;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const int tiles_x = (s.W + kTileW - 1) / kTileW, tiles_y = (s.H + kTileH - 1) / kTileH;
@@ -1063,15 +696,6 @@ cudaError_t launch_mlp_tc(const srcv_shape& s, const float* cur, const Workspace
   return err;
 }
 
-#ifdef SRCV_TC_TIMELINE
-}  // namespace srcv
-extern "C" int32_t srcv_debug_read_timeline(long long* host, int32_t n) {
-  const size_t bytes = sizeof(long long) * (size_t)(n < srcv::kTlTiles * srcv::kTlEvents ? n : srcv::kTlTiles * srcv::kTlEvents);
-  return (int32_t)cudaMemcpyFromSymbol(host, srcv::g_timeline, bytes);
-}
-namespace srcv {
-#endif
-
 // D (128 x 128) = A (128 x Kp) W^T (128 x Kp), Kp a multiple of 16 and <= 256; `scratch`
 // needs 2 * 128 * Kp halves.  Device pointers; test hook for tests/test_gpu_tc.py.
 cudaError_t launch_tc_selftest(const float* A, const float* Wm, int Kp, float* Dout, void* scratch,
@@ -1081,10 +705,10 @@ cudaError_t launch_tc_selftest(const float* A, const float* Wm, int Kp, float* D
   __half* lo = hi + (size_t)kN * Kp;
   SRCV_LAUNCH(tc_selftest_pack, 32, 256, 0, stream, Wm, Kp, hi, lo);
   note_launch();
-  const size_t smem = (size_t)2 * kN * Kp * 2;
+  const size_t smem = (size_t)2 * (kN + kRows) * Kp * 2;
   cudaError_t err = cudaFuncSetAttribute(tc_selftest_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
   if (err != cudaSuccess) return err;
-  SRCV_LAUNCH(tc_selftest_kernel, 1, 160, smem, stream, A, hi, lo, Kp, Dout);
+  SRCV_LAUNCH(tc_selftest_kernel, 1, 128, smem, stream, A, hi, lo, Kp, Dout);
   note_launch();
   return cudaGetLastError();
 }

@@ -1,17 +1,17 @@
-// Thin inline-PTX layer over the Blackwell tensor-core path used by the
-// metadata-MLP sweep: tcgen05.mma with the A operand in tensor memory (TMEM), the
-// B operand (weights) in shared memory, fp32 accumulators in TMEM, mbarrier
-// completion, tcgen05.ld/st for the thread<->TMEM traffic.  sm_100a only.
+// Thin inline-PTX layer over the Hopper tensor-core path used by the metadata-MLP sweep:
+// warpgroup MMAs (wgmma.mma_async, fp16 operands, fp32 accumulators in registers) with the
+// B operand (weights) and optionally the A operand in shared memory, mbarrier hand-offs
+// between warp roles, and the bulk-copy (TMA) engine for the weight image.  sm_90a.
 //
 // Layout conventions used here
-//   * TMEM address = (lane << 16) | column; a warp may touch lanes
-//     32*(warp_id % 4) .. +31 only; thread i of the warp owns lane base+i and the
-//     .32x32b.xN shapes move N consecutive 32-bit columns of that lane.
-//   * kind::f16 operands in TMEM: one 32-bit column holds two consecutive K elements
-//     (even K in the low half).  An MMA with K = 16 consumes 8 columns.
-//   * B operand: K-major, no swizzle ("interleave") canonical layout — 8 rows x 16
+//   * shared-memory operands: K-major, no swizzle ("interleave") canonical layout — 8 rows x 16
 //     bytes core matrices; row r, K chunk c (8 halves) lives at
 //         c * LBO + (r / 8) * SBO + (r % 8) * 16   bytes from the start address.
+//   * accumulator fragment of an m64nN wgmma (warp w of the warpgroup, lane = 4 g + q):
+//         d[4 j + e] = D[16 w + g + 8 (e / 2)][8 j + 2 q + (e % 2)]
+//   * register A fragment of one k16 step (same g, q):  a0 = row g, k 2q..2q+1;  a1 = row g + 8;
+//     a2 = row g, k 8 + 2q..;  a3 = row g + 8, k 8 + 2q..  (even k in the low half), i.e. exactly
+//     the packed accumulator words d[8 s .. 8 s + 7] of columns 16 s .. 16 s + 15 of an earlier layer.
 #pragma once
 #ifdef SRCV_HOST_EMU
 #include "emu_tc.h"   // tests/emu: functional host model of this layer (same names, same semantics)
@@ -50,7 +50,7 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
         : "memory");
   } while (!done);
 }
-// ---- bulk asynchronous copy global -> shared (TMA engine, UBLKCP), completion on an mbarrier
+// ---- bulk asynchronous copy global -> shared (TMA engine), completion on an mbarrier
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes)
                : "memory");
@@ -68,132 +68,65 @@ __device__ __forceinline__ void fence_proxy_async_smem() {
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
 
-// ---- TMEM allocation (one full warp) -----------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)),
-               "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-
-// ---- ordering ------------------------------------------------------------------------
-__device__ __forceinline__ void fence_before_sync() {
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void fence_after_sync() {
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-}
-__device__ __forceinline__ void wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-// all previously issued MMAs of this thread complete -> one arrival on `bar`
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(
-                   smem_u32(bar))
-               : "memory");
-}
-
 // ---- descriptors --------------------------------------------------------------------
-// shared-memory operand descriptor, K-major, no swizzle (see header comment)
+// shared-memory operand descriptor, K-major, no swizzle (see header comment); bits [62,64) = 0
 __device__ __forceinline__ uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);               // start address  [0,14)
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;      // leading offset [16,30)
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;      // stride offset  [32,46)
-  d |= static_cast<uint64_t>(1) << 46;                               // descriptor version (Blackwell)
-  return d;                                                          // layout_type [61,64) = 0: no swizzle
-}
-// instruction descriptor: kind::f16, A/B = f16 (K-major), D = f32, M x N
-__host__ __device__ constexpr uint32_t idesc_f16_f32(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
+  return d;
 }
 
-// One thread of a CONVERGED warp, chosen by elect.sync: code guarded by this predicate is known
-// to ptxas to run in a single thread, so a tcgen05.mma inside it is emitted bare — under a
-// `lane == 0` branch every MMA is wrapped in an ELECT / branch loop of its own (six dependent
-// instructions per MMA, which made the 128 x 128 x 16 MMAs issue-bound at ~87 clk against a
-// 64 clk tensor-pipe floor; scripts/mma_probe.cu, profiles/r02_mma_probe.jsonl).
-__device__ __forceinline__ bool elect_one() {
-  uint32_t pred;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "elect.sync _|p, 0xffffffff;\n\t"
-      "selp.u32 %0, 1, 0, p;\n\t}"
-      : "=r"(pred));
-  return pred != 0;
+// ---- warpgroup MMA (all 128 threads of an aligned warpgroup) --------------------------------
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void wgmma_wait() {
+  asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory");
+}
+// keeps the compiler from moving accumulator registers across the asynchronous MMAs
+template <int N> __device__ __forceinline__ void fence_regs(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
 
-// ---- MMA: D[tmem] (+)= A[tmem] * B[smem]^T ; issued by ONE thread -----------------------
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc,
-                                       uint32_t accumulate) {
+// D[64 x 128] (+)= A[smem, 64 x 16] B[smem, 128 x 16]^T
+__device__ __forceinline__ void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
-      : "memory");
-}
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc,
-                                       uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, {%5, %5, %5, %5}, p;\n\t}"
-      :
-      : "r"(d_tmem), "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate), "r"(0u)
+      "setp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, "
+      "%43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+      "%64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+        "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+        "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+        "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+        "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
 
-// ---- thread <-> TMEM ---------------------------------------------------------------------
-__device__ __forceinline__ void st_x1(uint32_t taddr, uint32_t r0) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x1.b32 [%0], {%1};" ::"r"(taddr), "r"(r0) : "memory");
-}
-__device__ __forceinline__ void st_x2(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x2.b32 [%0], {%1, %2};" ::"r"(taddr), "r"(r[0]), "r"(r[1]) : "memory");
-}
-__device__ __forceinline__ void st_x4(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(r[0]),
-               "r"(r[1]), "r"(r[2]), "r"(r[3])
-               : "memory");
-}
-__device__ __forceinline__ void st_x8(uint32_t taddr, const uint32_t* r) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr),
-               "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7])
-               : "memory");
-}
-__device__ __forceinline__ void st_x16(uint32_t taddr, const uint32_t* r) {
+// D[64 x 64] (+)= A[registers, 64 x 16] B[smem, 64 x 16]^T
+__device__ __forceinline__ void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc,
+                                             uint32_t accumulate) {
   asm volatile(
-      "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-      "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]),
-      "r"(r[9]), "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
-      : "memory");
-}
-__device__ __forceinline__ void ld_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void ld_x32(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-        "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]),
-        "=r"(r[15]), "=r"(r[16]), "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]),
-        "=r"(r[22]), "=r"(r[23]), "=r"(r[24]), "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]),
-        "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, "
+      "%22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+      "{%32, %33, %34, %35}, %36, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+        "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
 
@@ -215,19 +148,11 @@ __device__ __forceinline__ uint32_t pack_f16x2_sat(float even, float odd) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(d) : "f"(odd), "f"(even));  // {upper, lower}
   return d;
 }
-// The residual x - hi is one mixed-precision FMA per value (fma.rn.f32.f16: hi * (-1) + x, SASS
-// FHFMA with an .H0 / .H1 selector on the packed word) — four instructions per PAIR of values.
+// The residual x - hi is one mixed-precision FMA per value (fma.rn.f32.f16: hi * (-1) + x).
 __device__ __forceinline__ void split_pack(float even, float odd, uint32_t& hi, uint32_t& lo) {
   hi = pack_f16x2_sat(even, odd);
-  float re, ro;
-  asm("{\n\t.reg .b16 h0, h1, m1;\n\t"
-      "mov.b32 {h0, h1}, %2;\n\t"
-      "mov.b16 m1, 0xBC00;\n\t"               // -1.0 in fp16
-      "fma.rn.f32.f16 %0, h0, m1, %3;\n\t"
-      "fma.rn.f32.f16 %1, h1, m1, %4;\n\t}"
-      : "=f"(re), "=f"(ro)
-      : "r"(hi), "f"(even), "f"(odd));
-  lo = pack_f16x2_sat(re, ro);
+  const float2 h = __half22float2(*reinterpret_cast<const __half2*>(&hi));
+  lo = pack_f16x2_sat(even - h.x, odd - h.y);
 }
 
 }  // namespace tc

@@ -4,7 +4,7 @@
 ``FastFeatureVolumeManager`` in the reference's ``modules.cost_volume`` namespace
 (and in ``experiment_modules.depth_model`` if it was already imported, because it
 binds the names at import time — reference experiment_modules/depth_model.py:10-11)
-so ``DepthModel`` builds the sm_100a-backed classes without any edit to the
+so ``DepthModel`` builds the sm_90a-backed classes without any edit to the
 reference.  ``install(losses=True)`` also swaps the reference's ``losses.MVDepthLoss`` (the
 training loss of depth_model.py:144, :477-485) for the kernel-backed mirror.  See INTEGRATION.md.
 """

@@ -1,4 +1,4 @@
-"""Multi-view depth regression loss, backed by the sm_100a kernel.
+"""Multi-view depth regression loss, backed by the sm_90a kernel.
 
 Mirrors ``MVDepthLoss`` of the reference's ``losses.py`` (:79-208) — constructor ``(height, width)``,
 ``forward`` with the reference's keyword names (``experiment_modules/depth_model.py:477-485`` calls it
@@ -8,7 +8,7 @@ can construct it in place of the reference class.  The loss is differentiable w.
 and the cameras are data).
 
 One forward launch (+ a fixed-order finalize) walks all source views per pixel in registers; the
-backward is one launch that recomputes the geometry.  CUDA tensors on an sm_100 device, or an
+backward is one launch that recomputes the geometry.  CUDA tensors on an sm_90 device, or an
 exception: there is no CPU path.  Half / bfloat16 inputs (Lightning ``precision=16``) are computed in
 fp32, the gradient is returned in the prediction's dtype.
 """
@@ -25,7 +25,7 @@ from . import _native
 def _require_cuda(t: torch.Tensor) -> None:
     """The device gate (tests/ patch exactly this to drive the host-emulated library)."""
     if t.device.type != "cuda":
-        raise RuntimeError("simplerecon_b200 MVDepthLoss runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("simplerecon_b200 MVDepthLoss runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 def _lib():

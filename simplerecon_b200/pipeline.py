@@ -1,8 +1,9 @@
 """Host-to-host streaming of frame batches through a cost-volume manager.
 
-The sweep itself takes ~0.1 ms per frame on a B200 while moving a frame's inputs
-(9.8 MB) and outputs (5 MB) over PCIe takes ~0.3 ms, so a caller whose tuples start in
-host memory is transfer-bound unless the three legs overlap.  ``HostStreamer`` runs
+The dot-product sweep itself takes ~0.11 ms per frame on an H100 (SXM, 700 W) while moving a
+frame's inputs (9.8 MB) and outputs (5 MB) over PCIe takes longer (~0.2 ms per frame end to end
+on the same card, with the legs overlapped), so a caller whose tuples start in host memory is
+transfer-bound unless the three legs overlap.  ``HostStreamer`` runs
 
     H2D(batch i+1)  ||  sweep(batch i)  ||  D2H(batch i-1)
 

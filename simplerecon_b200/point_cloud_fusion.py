@@ -1,4 +1,4 @@
-"""Multi-view depth-consistency point-cloud fusion, backed by the sm_100a kernel.
+"""Multi-view depth-consistency point-cloud fusion, backed by the sm_90a kernel.
 
 Mirrors the reference's ``tools/torch_point_cloud_fusion.py`` — ``process_depth`` (:12-97) and
 ``process_scene`` (:100-118), the 3DVNet-style fuser ``pc_fusion.py:158`` calls — with the same
@@ -6,7 +6,7 @@ names, argument meaning and return values (numpy arrays of the consistent points
 and the per-pixel validity), so ``pc_fusion.py`` can import this module in its place.
 
 One launch per reference frame walks every source frame in registers (the reference materialises
-(n_src, 3, H*W) tensors several times over per batch of 100 sources).  CUDA tensors on an sm_100
+(n_src, 3, H*W) tensors several times over per batch of 100 sources).  CUDA tensors on an sm_90
 device, or an exception: there is no CPU path.
 """
 from __future__ import annotations
@@ -22,7 +22,7 @@ from . import _native
 def _require_cuda(t: torch.Tensor) -> None:
     """The device gate (tests/ patch exactly this to drive the host-emulated library)."""
     if t.device.type != "cuda":
-        raise RuntimeError("simplerecon_b200 point-cloud fusion runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("simplerecon_b200 point-cloud fusion runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 class _Scan:

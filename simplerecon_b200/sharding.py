@@ -3,7 +3,7 @@
 Every reference frame (batch element) is an independent unit — all reductions of
 the sweep are over channels, views and planes *within* a frame — so the path
 shards by frame with NO data-path collective.  ``torch.distributed`` (NCCL over
-NVLink on the GPU box, gloo in the CPU tests) is used only for the barrier around
+NVLink between GPUs, gloo in the CPU tests) is used only for the barrier around
 the timed region, the MAX-reduce of the elapsed time and, optionally, gathering
 results for a global check.
 """

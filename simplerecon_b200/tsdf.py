@@ -1,4 +1,4 @@
-"""Dense-grid TSDF fusion of predicted depth maps, backed by the sm_100a kernel.
+"""Dense-grid TSDF fusion of predicted depth maps, backed by the sm_90a kernel.
 
 Mirrors the reference's ``tools/tsdf.py`` — ``TSDF`` (:11-170, the volume and its bounds
 arithmetic) and ``TSDFFuser`` (:173-320, ``integrate_depth``) — as ``OurFuser.fuse_frames``
@@ -10,7 +10,7 @@ reference's.
 Differences, by design: ``voxel_coords`` is not stored (the kernel recomputes the 6 bytes per
 voxel from the grid index; the property materialises it on demand), a batch of frames is ONE
 launch (frames are applied in order inside the kernel), and there is no CPU path: CUDA tensors
-on an sm_100 device, or an exception.
+on an sm_90 device, or an exception.
 """
 from __future__ import annotations
 
@@ -74,7 +74,7 @@ class TSDF:
 def _require_cuda(t: torch.Tensor) -> None:
     """The device gate of the fuser (tests/ patch exactly this to drive the host-emulated library)."""
     if t.device.type != "cuda":
-        raise RuntimeError("simplerecon_b200 TSDF fusion runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("simplerecon_b200 TSDF fusion runs on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 class TSDFFuser:

@@ -10,7 +10,7 @@ REPO = HERE.parent.parent
 BUILD = HERE / "_build"
 CXX = "/usr/bin/g++" if Path("/usr/bin/g++").is_file() else "g++"
 CSRC = REPO / "simplerecon_b200" / "csrc"
-# every kernel file (the tcgen05 one against the functional model in emu_tc.h) plus the C-ABI front end
+# every kernel file (the wgmma one against the functional model in emu_tc.h) plus the C-ABI front end
 UNITS = [CSRC / n for n in ("srcv_api.cu", "srcv_prep.cu", "srcv_dot.cu", "srcv_dot_bwd.cu",
                             "srcv_mlp_generic.cu", "srcv_mlp_bwd.cu", "srcv_mlp_tc.cu", "srcv_tsdf.cu", "srcv_producer.cu", "srcv_mvs.cu", "srcv_mvloss.cu")]
 SOURCES = [HERE / "emu_driver.cpp", HERE / "emu_cuda.h", HERE / "emu_tc.h", REPO / "include" / "srcv_b200.h", *sorted(CSRC.glob("*"))]

@@ -8,7 +8,8 @@
 // atomics as real host atomics.  It exists so that indexing, barrier placement and the
 // arithmetic of a kernel can be checked against the oracle in the CPU test tier, before any
 // GPU time is spent; it says nothing about launch limits, registers or speed.
-// Not emulated: warp-level intrinsics, tcgen05 / TMA / mbarrier (those kernels are GPU-only).
+// Warp-level intrinsics: __shfl_sync / __shfl_xor_sync / __all_sync over full, converged warps.
+// The wgmma / mbarrier / bulk-copy layer is modelled in emu_tc.h.
 #pragma once
 #include <atomic>
 #include <barrier>
@@ -39,11 +40,11 @@ enum cudaFuncAttribute { cudaFuncAttributeMaxDynamicSharedMemorySize };
 namespace emu { inline int g_sms = 4; }   // "SM count" the launch heuristics see (emu_set_sms)
 inline cudaError_t cudaGetDevice(int* d) { *d = 0; return cudaSuccess; }
 inline cudaError_t cudaDeviceGetAttribute(int* v, cudaDeviceAttr a, int) {
-  *v = (a == cudaDevAttrComputeCapabilityMajor) ? 10 : ::emu::g_sms;
+  *v = (a == cudaDevAttrComputeCapabilityMajor) ? 9 : ::emu::g_sms;
   return cudaSuccess;
 }
 template <class K> inline cudaError_t cudaFuncSetAttribute(K, cudaFuncAttribute, int bytes) {
-  return bytes <= 227 * 1024 ? cudaSuccess : cudaErrorInvalidValue;   // the sm_100 opt-in limit
+  return bytes <= 227 * 1024 ? cudaSuccess : cudaErrorInvalidValue;   // the sm_90 opt-in limit
 }
 inline cudaError_t cudaGetLastError() { return cudaSuccess; }
 inline const char* cudaGetErrorName(cudaError_t) { return "emuError"; }
@@ -77,7 +78,6 @@ struct WarpVote {
   std::atomic<int> acc[3];
 };
 inline thread_local WarpVote* t_votes = nullptr;
-inline thread_local uint32_t* t_tmem = nullptr;        // tensor memory of the CTA (emu_tc.h)
 inline thread_local uint32_t* t_shfl = nullptr;        // per-warp exchange slots for __shfl_sync
 inline thread_local unsigned t_vote_round = 0;
 
@@ -91,7 +91,7 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, F&& body) {
       for (unsigned bx = 0; bx < grid.x; ++bx) {
         void* sm = std::aligned_alloc(1024, ((bytes + 1023) / 1024) * 1024);
         std::memset(sm, 0xFF, bytes);
-        std::vector<uint32_t> tmem(128 * 512, 0xFFFFFFFFu), shfl(((nthreads + 31) / 32) * 32, 0u);  // all-ones = NaN as float: uninitialised reads poison the result
+        std::vector<uint32_t> shfl(((nthreads + 31) / 32) * 32, 0u);
         std::barrier<> bar((std::ptrdiff_t)nthreads);
         const unsigned nwarps = (nthreads + 31) / 32;
         std::vector<WarpVote> votes(nwarps);
@@ -112,7 +112,6 @@ void launch(dim3 grid, dim3 block, size_t smem_bytes, F&& body) {
             t_smem = sm;
             t_bar = &bar;
             t_votes = votes.data();
-            t_tmem = tmem.data();
             t_shfl = shfl.data();
             t_vote_round = 0;
             body();
@@ -175,6 +174,10 @@ inline int __shfl_sync(unsigned, int v, int src_lane) {
   const int r = (int)slots[src_lane & 31];
   w.bar->arrive_and_wait();                 // nobody overwrites a slot before everybody has read
   return r;
+}
+inline float __shfl_xor_sync(unsigned m, float v, int lane_mask) {
+  const int lane = (int)((threadIdx.x + blockDim.x * (threadIdx.y + blockDim.y * threadIdx.z)) & 31u);
+  return __uint_as_float((unsigned)__shfl_sync(m, (int)__float_as_uint(v), lane ^ lane_mask));
 }
 
 // __all_sync over a full, converged warp (the only warp-level intrinsic the SIMT kernels use):

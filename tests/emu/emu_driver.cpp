@@ -3,7 +3,7 @@
 // tests/emu/__init__.py compiles the product's own sources (every csrc/*.cu) as host C++ with
 // -DSRCV_HOST_EMU and links them with this file into tests/emu/_build/libsrcv_emu.so, which
 // therefore exports the SAME entry points as include/srcv_b200.h, taking HOST pointers.  The
-// tcgen05 kernel runs against the functional TMEM / MMA / mbarrier model of emu_tc.h.
+// wgmma kernel runs against the functional wgmma / mbarrier model of emu_tc.h.
 #define SRCV_HOST_EMU 1
 #include "../../simplerecon_b200/csrc/srcv_kernels.h"
 

@@ -1,24 +1,16 @@
-// Host emulation of the tcgen05 / TMEM / mbarrier / bulk-copy layer of csrc/srcv_tc.cuh —
+// Host emulation of the wgmma / mbarrier / bulk-copy layer of csrc/srcv_tc.cuh —
 // TEST INFRASTRUCTURE (see emu_cuda.h).  Same function names and argument meaning as the
-// inline-PTX wrappers, with the FUNCTIONAL semantics the GPU-validated kernel relies on:
+// inline-PTX wrappers, with the FUNCTIONAL semantics the GPU kernel relies on:
 //
-//   * tensor memory: 128 lanes x 512 32-bit columns per CTA (NaN-poisoned); address =
-//     (lane << 16) | column; a .32x32b access of thread i touches lane (addr.lane + i % 32);
-//   * tcgen05.mma.kind::f16, M = 128: D[m][n] (+)= sum_{k<16} A[m][k] B[n][k], A from TMEM (two
-//     K elements per column, even K in the low half) or from shared memory, B from shared
-//     memory through a K-major no-swizzle descriptor (start, LBO, SBO in 16-byte units);
-//     products are exact, accumulation is fp32 in k order (the hardware's order is not
-//     specified: results agree to rounding, not bit for bit);
-//   * MMAs are queued by the issuing thread and EXECUTED AT tcgen05.commit, just before the
-//     commit's mbarrier arrival — i.e. as late as the hardware is allowed to run them, so that
-//     an operand overwritten between issue and commit corrupts the result here too;
+//   * wgmma m64nNk16 f16 -> f32: each thread computes its own accumulator fragment (layout in
+//     srcv_tc.cuh); A from a K-major no-swizzle smem descriptor or from the quad's registers (via
+//     __shfl_sync), B from smem; exact products, fp32 accumulation in k order;
+//   * MMAs execute at issue; commit / wait / fences are no-ops (the kernels wait right after each commit);
 //   * mbarrier: phase bit | pending arrivals | arrival count | pending transaction bytes packed
 //     in the 64-bit word, updated with CAS; waits block on the word (std::atomic_ref::wait).
 //     Acquire/release on the word gives ThreadSanitizer the happens-before edges of the real
-//     protocol: a TMEM / shared-memory hand-off that is not ordered by a barrier is a data race.
-//   * tcgen05.fence / wait::ld / wait::st / proxy fences: no-ops (program order on the host).
-// Not modelled: asynchrony of tcgen05.st / ld (so a missing tcgen05.wait is not detected),
-// cta_group::2, swizzled layouts, multicast.
+//     protocol: a shared-memory hand-off that is not ordered by a barrier is a data race.
+// Not modelled: the asynchrony of wgmma, swizzled layouts, clusters, setmaxnreg.
 #pragma once
 #include "emu_cuda.h"
 
@@ -86,56 +78,22 @@ inline void bulk_g2s(void* smem_dst, const void* gmem_src, uint32_t bytes, uint6
 }
 inline void fence_proxy_async_smem() {}
 
-// ---- tensor memory --------------------------------------------------------------------------
-constexpr int kTmemLanes = 128, kTmemColumns = 512;
-inline uint32_t* tmem_cell(uint32_t taddr, int lane_off, int n) {
-  const uint32_t lane = (taddr >> 16) + (uint32_t)lane_off, col = taddr & 0xFFFFu;
-  if (lane >= (uint32_t)kTmemLanes || col + (uint32_t)n > (uint32_t)kTmemColumns) {
-    std::fprintf(stderr, "emu: TMEM access out of range (lane %u, columns %u..%u)\n", lane, col, col + n);
-    std::abort();
-  }
-  return ::emu::t_tmem + (size_t)lane * kTmemColumns + col;
-}
-inline void tmem_alloc(uint32_t* smem_dst, uint32_t) { if ((threadIdx.x & 31) == 0) *smem_dst = 0u; }
-inline void tmem_dealloc(uint32_t, uint32_t) {}
-inline void fence_before_sync() {}
-inline void fence_after_sync() {}
-inline void wait_ld() {}
-inline void wait_st() {}
-
-template <int N> inline void st_n(uint32_t taddr, const uint32_t* r) {
-  uint32_t* c = tmem_cell(taddr, threadIdx.x & 31, N);
-  for (int j = 0; j < N; ++j) c[j] = r[j];
-}
-template <int N> inline void ld_n(uint32_t taddr, uint32_t* r) {
-  const uint32_t* c = tmem_cell(taddr, threadIdx.x & 31, N);
-  for (int j = 0; j < N; ++j) r[j] = c[j];
-}
-inline void st_x1(uint32_t taddr, uint32_t r0) { st_n<1>(taddr, &r0); }
-inline void st_x2(uint32_t taddr, const uint32_t* r) { st_n<2>(taddr, r); }
-inline void st_x4(uint32_t taddr, const uint32_t* r) { st_n<4>(taddr, r); }
-inline void st_x8(uint32_t taddr, const uint32_t* r) { st_n<8>(taddr, r); }
-inline void st_x16(uint32_t taddr, const uint32_t* r) { st_n<16>(taddr, r); }
-inline void ld_x16(uint32_t taddr, uint32_t* r) { ld_n<16>(taddr, r); }
-inline void ld_x32(uint32_t taddr, uint32_t* r) { ld_n<32>(taddr, r); }
-
 // ---- descriptors (bit-identical to the device versions) -------------------------------------
 inline uint64_t smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((saddr & 0x3FFFFu) >> 4);
   d |= static_cast<uint64_t>((lbo_bytes >> 4) & 0x3FFFu) << 16;
   d |= static_cast<uint64_t>((sbo_bytes >> 4) & 0x3FFFu) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
   return d;
 }
-constexpr uint32_t idesc_f16_f32(int M, int N) {
-  return (1u << 4) | (static_cast<uint32_t>(N >> 3) << 17) | (static_cast<uint32_t>(M >> 4) << 24);
-}
 
-// ---- MMA ------------------------------------------------------------------------------------
+// ---- warpgroup MMA ---------------------------------------------------------------------------
+inline void wgmma_fence() {}
+inline void wgmma_commit() {}
+template <int N> inline void wgmma_wait() {}
+template <int N> inline void fence_regs(float (&)[N]) {}
+
 namespace detail {
-struct Mma { uint32_t d; bool a_in_tmem; uint32_t a_tmem; uint64_t a_desc, b_desc; uint32_t idesc, acc; };
-inline thread_local std::vector<Mma> t_queue;
 inline float half_bits(uint16_t h) { _Float16 f; std::memcpy(&f, &h, 2); return (float)f; }
 inline const char* operand(uint64_t desc, int row, int k) {       // K-major, no swizzle, 8 x 16-byte core matrices
   const uint32_t start = (uint32_t)(desc & 0x3FFFu) << 4, lbo = (uint32_t)((desc >> 16) & 0x3FFFu) << 4,
@@ -143,50 +101,46 @@ inline const char* operand(uint64_t desc, int row, int k) {       // K-major, no
   return reinterpret_cast<const char*>(::emu::dynamic_smem()) + start + (uint32_t)(k >> 3) * lbo +
          (uint32_t)(row >> 3) * sbo + (uint32_t)(row & 7) * 16u + (uint32_t)(k & 7) * 2u;
 }
-inline void execute(const Mma& m) {
-  const int M = (int)((m.idesc >> 24) & 0x1Fu) << 4, N = (int)((m.idesc >> 17) & 0x3Fu) << 3;
-  if (M != 128) { std::fprintf(stderr, "emu: only M = 128 MMAs are modelled\n"); std::abort(); }
-  for (int r = 0; r < M; ++r) {
-    float a[16];
-    for (int k = 0; k < 16; ++k) {
-      uint16_t h;
-      if (m.a_in_tmem) {
-        const uint32_t w = *tmem_cell(m.a_tmem + (uint32_t)(k >> 1), r, 1);
-        h = (uint16_t)(w >> (16 * (k & 1)));
-      } else {
-        std::memcpy(&h, operand(m.a_desc, r, k), 2);
-      }
-      a[k] = half_bits(h);
+inline float operand_value(uint64_t desc, int row, int k) {
+  uint16_t h;
+  std::memcpy(&h, operand(desc, row, k), 2);
+  return half_bits(h);
+}
+inline int warp_in_group() { return (int)(((threadIdx.x + blockDim.x * (threadIdx.y + blockDim.y * threadIdx.z)) / 32) & 3u); }
+// the N / 2 fragment elements of this thread: rows[0] = A row 16 w + g, rows[1] = A row 16 w + g + 8
+template <int N>
+inline void mma_fragment(float* d, const float (&rows)[2][16], uint64_t b_desc, uint32_t acc) {
+  const int q = (int)(threadIdx.x & 3u);
+  for (int j = 0; j < N / 8; ++j)
+    for (int e = 0; e < 4; ++e) {
+      const int n = 8 * j + 2 * q + (e & 1);
+      float s = acc ? d[4 * j + e] : 0.f;
+      for (int k = 0; k < 16; ++k) s += rows[e >> 1][k] * operand_value(b_desc, n, k);
+      d[4 * j + e] = s;
     }
-    uint32_t* drow = tmem_cell(m.d, r, N);
-    for (int n = 0; n < N; ++n) {
-      float s;
-      if (m.acc) std::memcpy(&s, &drow[n], 4); else s = 0.f;
-      for (int k = 0; k < 16; ++k) {
-        uint16_t h;
-        std::memcpy(&h, operand(m.b_desc, n, k), 2);
-        s += a[k] * half_bits(h);
-      }
-      std::memcpy(&drow[n], &s, 4);
-    }
-  }
 }
 }  // namespace detail
 
-inline void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  detail::t_queue.push_back(detail::Mma{d_tmem, true, a_tmem, 0, b_desc, idesc, accumulate});
+inline void wgmma_ss_n128(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
+  const int r0 = 16 * detail::warp_in_group() + (int)((threadIdx.x & 31u) >> 2);
+  float rows[2][16];
+  for (int h = 0; h < 2; ++h)
+    for (int k = 0; k < 16; ++k) rows[h][k] = detail::operand_value(a_desc, r0 + 8 * h, k);
+  detail::mma_fragment<128>(d, rows, b_desc, accumulate);
 }
-inline void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  detail::t_queue.push_back(detail::Mma{d_tmem, false, 0, a_desc, b_desc, idesc, accumulate});
+inline void wgmma_rs_n64(float (&d)[32], const uint32_t (&a)[4], uint64_t b_desc, uint32_t accumulate) {
+  // a0: row g, k 2q, 2q+1;  a1: row g+8;  a2: row g, k 8+2q, 9+2q;  a3: row g+8  (q = the source lane of the quad)
+  const int g = (int)((threadIdx.x & 31u) >> 2);
+  float rows[2][16];
+  for (int src = 0; src < 4; ++src)
+    for (int i = 0; i < 4; ++i) {
+      const uint32_t w = (uint32_t)__shfl_sync(0xffffffffu, (int)a[i], 4 * g + src);
+      const int h = i & 1, k = 2 * src + 8 * (i >> 1);
+      rows[h][k] = detail::half_bits((uint16_t)w);
+      rows[h][k + 1] = detail::half_bits((uint16_t)(w >> 16));
+    }
+  detail::mma_fragment<64>(d, rows, b_desc, accumulate);
 }
-inline void mma_commit(uint64_t* bar) {
-  for (const auto& m : detail::t_queue) detail::execute(m);
-  detail::t_queue.clear();
-  detail::update(bar, 1, 0);
-}
-
-// elect.sync of a converged warp: the model always picks lane 0
-inline bool elect_one() { return (threadIdx.x & 31) == 0; }
 
 template <int N> inline void reg_inc() {}
 template <int N> inline void reg_dec() {}

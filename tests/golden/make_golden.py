@@ -1,6 +1,6 @@
 """Generates the golden vectors in tests/golden/*.npz from the UNMODIFIED reference.
 
-Run in the build container (needs /root/reference):
+Needs the SimpleRecon source tree ($SIMPLERECON_REF):
 
     python tests/golden/make_golden.py
 

@@ -1,6 +1,6 @@
 """Golden vectors at the BENCH feature-map size (120 x 160, 7 views) from the UNMODIFIED reference.
 
-    python tests/golden/make_golden_fullsize.py          (build container: needs /root/reference)
+    python tests/golden/make_golden_fullsize.py          (needs $SIMPLERECON_REF)
 
 The fixtures of make_golden.py top out at 48 x 64, so they never reach the kernels' compile-time
 160 x 120 instantiations.  At this size the inputs (8.6 MB of source features per frame) are too large

@@ -53,7 +53,7 @@ def test_mlp_flops_match_survey_and_configs_agree_between_arms():
     # SURVEY.md §8(d): 104.1 GFLOP (MLP) per frame at cfgA, 156.2 at cfgB
     assert abs(bench.mlp_flops_per_frame(CONFIGS[2], False) - 104.1e9) < 0.1e9
     assert abs(bench.mlp_flops_per_frame(CONFIGS[3], False) - 156.2e9) < 0.15e9
-    # what the tcgen05 kernel issues: 3 MMAs per product, layer-1 K = 192 (pose measures as a bias)
+    # what the wgmma kernel issues: 3 MMAs per product, layer-1 K = 192 (pose measures as a bias)
     assert bench.mlp_flops_per_frame(CONFIGS[2], True) > 3 * 0.95 * bench.mlp_flops_per_frame(CONFIGS[2], False)
     # the default workload is the hero configuration at 8 frames per GPU: N = 1 is BASELINE configs[2],
     # N = 8 is configs[4]; both arms print the same `config`

@@ -10,6 +10,7 @@ import torch
 
 import simplerecon_b200 as S
 from simplerecon_b200.synthetic import CONFIGS, make_tuple, mlp_state
+from tests import refgolden
 
 FWD_ARGS = ["self", "cur_feats", "src_feats", "src_extrinsics", "src_poses", "src_Ks", "cur_invK",
             "min_depth", "max_depth", "depth_planes_bdhw", "return_mask"]
@@ -149,19 +150,51 @@ def test_synthetic_tuples_are_deterministic_and_shaped():
         ("mlp", 16, 7, 120, 160, 96), ("mlp", 64, 7, 120, 160, 64)]
 
 
-def test_install_against_the_real_reference_module():
-    """install() on the UNMODIFIED reference's modules.cost_volume (build container only): the
-    three names resolve to our classes, `isinstance` / `to_fast()` as used by test.py:196-198 keep
-    working, a state_dict produced by the reference class loads strictly into ours, and
-    uninstall() restores the reference."""
-    from oracle.ref_import import load_reference, reference_available
-    if not reference_available():
-        pytest.skip("reference tree not mounted")
+_CV_NAMES = ("CostVolumeManager", "FeatureVolumeManager", "FastFeatureVolumeManager")
+_LOSS_METHODS = ("__init__", "forward", "get_valid_mask", "get_error_for_pair")
+
+
+def reference_outputs():
+    """The surface of the reference modules install() patches, recorded from the unmodified tree
+    (tests/golden/make_reference_golden.py): the strict state_dict of its FeatureVolumeManager
+    (key -> shape) and the parameter lists of MVDepthLoss's methods."""
+    import importlib
+
+    import numpy as np
+
+    from oracle.ref_import import load_reference
     R = load_reference()
-    import modules.cost_volume as ref_cv          # importable once load_reference() put the tree on sys.path
-    orig = {n: getattr(ref_cv, n) for n in ("CostVolumeManager", "FeatureVolumeManager", "FastFeatureVolumeManager")}
-    ref_state = orig["FeatureVolumeManager"](12, 16, num_depth_bins=8, mlp_channels=[0, 128, 128, 1],
-                                             matching_dim_size=16, num_source_views=7).state_dict()
+    sd = R.FeatureVolumeManager(12, 16, num_depth_bins=8, mlp_channels=[0, 128, 128, 1], matching_dim_size=16,
+                                num_source_views=7).state_dict()
+    ref_losses = importlib.import_module("losses")
+    return {"state_dict": {k: torch.tensor(list(v.shape), dtype=torch.int64) for k, v in sd.items()},
+            "signature": {n: np.array(list(inspect.signature(getattr(ref_losses.MVDepthLoss, n)).parameters))
+                          for n in _LOSS_METHODS}}
+
+
+def _reference_modules(monkeypatch):
+    """Stand-ins for the reference's `modules.cost_volume` and `losses` under their import names:
+    install() finds them exactly where it finds the real ones in a SimpleRecon checkout."""
+    pkg, cv, losses = (types.ModuleType(n) for n in ("modules", "modules.cost_volume", "losses"))
+    pkg.cost_volume = cv
+    for n in _CV_NAMES:
+        setattr(cv, n, type(n, (torch.nn.Module,), {}))
+    losses.MVDepthLoss = type("MVDepthLoss", (torch.nn.Module,), {})
+    for name, mod in (("modules", pkg), ("modules.cost_volume", cv), ("losses", losses)):
+        monkeypatch.setitem(sys.modules, name, mod)
+    return cv, losses
+
+
+def test_install_against_the_real_reference_module(monkeypatch):
+    """install() on the reference's modules.cost_volume: the three names resolve to our classes,
+    `isinstance` / `to_fast()` as used by test.py:196-198 keep working, a state_dict shaped like the
+    reference class's (recorded) loads strictly into ours, and uninstall() restores the reference."""
+    ref_cv, _ = _reference_modules(monkeypatch)
+    orig = {n: getattr(ref_cv, n) for n in _CV_NAMES}
+    g = torch.Generator().manual_seed(0)
+    ref_state = {k: torch.randn(shape.tolist(), generator=g)
+                 for k, shape in refgolden.load("boundary", "state_dict").items()}
+    assert len(ref_state) == 9
     try:
         patched = S.install()
         assert "modules.cost_volume" in patched
@@ -176,29 +209,25 @@ def test_install_against_the_real_reference_module():
         fast = cv.to_fast()                                             # test.py:198
         assert isinstance(fast, ref_cv.FastFeatureVolumeManager) and fast.mlp is cv.mlp
         assert set(cv.state_dict()) == set(ref_state)
+        assert all(torch.equal(cv.state_dict()[k].cpu(), v) for k, v in ref_state.items())
     finally:
         S.uninstall()
     for n, c in orig.items():
         assert getattr(ref_cv, n) is c
 
 
-def test_install_swaps_the_real_reference_loss_class():
-    """install(losses=True) on the UNMODIFIED reference's losses module (build container only): MVDepthLoss
-    resolves to the kernel-backed mirror with the reference's constructor / forward / helper signatures;
-    uninstall() restores it."""
-    from oracle.ref_import import load_reference, reference_available
-    if not reference_available():
-        pytest.skip("reference tree not mounted")
-    load_reference()
-    import importlib
-    ref_losses = importlib.import_module("losses")
+def test_install_swaps_the_real_reference_loss_class(monkeypatch):
+    """install(losses=True) on the reference's losses module: MVDepthLoss resolves to the kernel-backed
+    mirror with the reference's (recorded) constructor / forward / helper signatures; uninstall() restores it."""
+    _, ref_losses = _reference_modules(monkeypatch)
     orig = ref_losses.MVDepthLoss
+    sig = refgolden.load("boundary", "signature")
+    assert set(sig) == set(_LOSS_METHODS)
     try:
         patched = S.install(losses=True)
         assert "losses" in patched and ref_losses.MVDepthLoss is S.MVDepthLoss
-        for name in ("__init__", "forward", "get_valid_mask", "get_error_for_pair"):
-            assert list(inspect.signature(getattr(S.MVDepthLoss, name)).parameters) == \
-                list(inspect.signature(getattr(orig, name)).parameters), name
+        for name in _LOSS_METHODS:
+            assert list(inspect.signature(getattr(S.MVDepthLoss, name)).parameters) == sig[name].tolist(), name
         loss = ref_losses.MVDepthLoss(192, 256)                     # depth_model.py:144-147
         assert loss.height == 192 and loss.width == 256
         with pytest.raises(RuntimeError):                           # CPU tensors: refused, no fallback

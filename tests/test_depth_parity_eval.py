@@ -1,4 +1,4 @@
-"""CPU half of the depth-map parity check: when a GPU run left gpurun_out/depth_parity_ours.npz
+"""CPU half of the depth-map parity check: when a GPU run left scripts/depth_parity.py's DUMP
 (tests/test_gpu_depth_parity.py) and the reference tree is mounted, push the reference's and our
 cost volumes through the reference's own CVEncoder + DepthDecoderPP (seeded weights) and require
 depth Abs-Diff <= 1e-4 on every frame (utils/metrics_utils.py:38; BASELINE.json north_star)."""
@@ -18,7 +18,7 @@ def test_depth_abs_diff_through_the_reference_unet():
     dp = importlib.util.module_from_spec(spec)
     spec.loader.exec_module(dp)
     if not dp.DUMP.is_file():
-        pytest.skip("no GPU dump (run tests/test_gpu_depth_parity.py through gpurun first)")
+        pytest.skip("no GPU dump (run tests/test_gpu_depth_parity.py on the GPU first)")
     import numpy as np
     z = np.load(dp.DUMP)
     if z["hero_cost"].shape[0] != dp.FRAMES["hero"] or z["dot_cost"].shape[0] != dp.FRAMES["dot"]:

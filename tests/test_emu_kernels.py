@@ -5,9 +5,9 @@ and checked against the oracle — kernel-source parity in the CPU tier.
 What this covers that the `-m gpu` tests cannot cover here (no GPU in this container):
 indexing, barrier placement, launch heuristics (plane-loop split + last-arriver argmax of the
 dot sweep, persistent grid of the MLP backward), workspace carving and argument validation of
-every entry point of include/srcv_b200.h — including the tcgen05 kernel, which runs against a
-functional model of TMEM / tcgen05.mma / mbarrier / bulk copy (tests/emu/emu_tc.h).  What it
-cannot cover: hardware limits, registers, speed, the asynchrony of tcgen05.ld/st — and device
+every entry point of include/srcv_b200.h — including the wgmma kernel, which runs against a
+functional model of wgmma / mbarrier / bulk copy (tests/emu/emu_tc.h).  What it
+cannot cover: hardware limits, registers, speed, the asynchrony of wgmma — and device
 intrinsics are replaced by IEEE host math, so tolerances are the parity tolerances of
 tests/parity.py, not bit-exactness.
 scripts/emu_sanitize.sh runs this file under ThreadSanitizer (shared-memory races) and
@@ -67,7 +67,7 @@ def test_golden_through_emulated_abi(lib, name, variant):
         wts = O.mlp_weights_from_state_dict(sd)
         cost, lowest, planes_bd, mask, used = emu.mlp_forward(inputs, D, wts, planes=planes_in)
     lib.srcv_set_variant(N.VARIANT_AUTO)
-    assert (("fast" in used) or ("tcgen05" in used)) == (variant == "auto"), used
+    assert (("fast" in used) or ("wgmma" in used)) == (variant == "auto"), used
     assert_cost_close(kind, cost, g["ref_cost"], g["ref_cost64"], what=f"emu {name}/{used}")
     planes = planes_in if planes_in is not None else planes_bd.view(B, D, 1, 1)
     if planes_in is None:
@@ -172,7 +172,7 @@ def test_warp_features(lib):
     (2, 3, 16, 9, 11, 2, (96, 64), True),
 ])
 def test_mlp_forward(lib, B, K, C, H, W, D, hidden, per_pixel):
-    lib.srcv_set_variant(N.VARIANT_GENERIC)         # the fp32 SIMT variant (the hero layout would pick tcgen05)
+    lib.srcv_set_variant(N.VARIANT_GENERIC)         # the fp32 SIMT variant (the hero layout would pick wgmma)
     t = make_tuple(B, K, H, W, channels=C, seed=21)
     wts = _weights(K, C, hidden)
     planes = (0.3 + 4.0 * torch.rand(B, D, H, W, generator=torch.Generator().manual_seed(22))) if per_pixel else None
@@ -218,10 +218,10 @@ def test_mlp_backward(lib, B, K, C, H, W, D, hidden, per_pixel, sms):
 
 
 # ----------------------------------------------------------------------------------------- #
-# tcgen05 kernel against the functional TMEM / MMA / mbarrier model (tests/emu/emu_tc.h)       #
+# wgmma kernel against the functional wgmma / mbarrier model (tests/emu/emu_tc.h)       #
 # ----------------------------------------------------------------------------------------- #
 def test_tc_selftest_three_product_gemm(lib):
-    """srcv_tc_selftest_f32: D = A W^T through tcgen05.mma with the (hi, lo) fp16 split."""
+    """srcv_tc_selftest_f32: D = A W^T through wgmma with the (hi, lo) fp16 split."""
     g = torch.Generator().manual_seed(0)
     for Kp, scale in ((64, 0.1), (208, 1.0)):
         A, Wm = torch.randn(128, Kp, generator=g), scale * torch.randn(128, Kp, generator=g)
@@ -234,13 +234,14 @@ def test_tc_selftest_three_product_gemm(lib):
 
 
 @pytest.mark.parametrize("B,H,W,D,per_pixel,sms", [
-    (1, 8, 16, 8, False, 2),      # 8 tiles over 2 persistent CTAs: the steady-state pipeline (prologue, overlap, drain)
-    (2, 5, 19, 6, False, 3),      # ragged patches (partial 16x2 tiles), D not a multiple of the 4-plane tile, 2 frames
+    (1, 8, 16, 8, False, 2),      # 16 tiles over 2 persistent CTAs: the steady-state pipeline (prologue, overlap, drain)
+    (2, 5, 19, 6, False, 3),      # ragged patches (partial 16x2 tiles), 2 frames
+    (2, 5, 19, 5, False, 3),      # ... and D not a multiple of the 2-plane tile
     (1, 6, 16, 4, True, 8),       # per-pixel planes; more CTAs than tiles per CTA > 1
 ])
-def test_mlp_forward_tcgen05(lib, B, H, W, D, per_pixel, sms):
-    """mlp_tc_kernel (K = 7, C = 16, 128/128): 640 host threads per CTA run the real worker / MMA-warp
-    code; TMEM, tcgen05.mma (executed at commit), mbarriers and the bulk copy are the functional
+def test_mlp_forward_wgmma(lib, B, H, W, D, per_pixel, sms):
+    """mlp_tc_kernel (K = 7, C = 16, 128/128): 512 host threads per CTA run the real builder / consumer-warpgroup
+    code; wgmma (executed at issue), mbarriers and the bulk copy are the functional
     model.  Checks the protocol (no deadlock, no lost tile) and the arithmetic against the oracle."""
     lib.emu_set_sms(sms)
     lib.srcv_set_variant(N.VARIANT_AUTO)
@@ -249,12 +250,12 @@ def test_mlp_forward_tcgen05(lib, B, H, W, D, per_pixel, sms):
     wts = _weights(K, C_)
     planes = (0.3 + 4.0 * torch.rand(B, D, H, W, generator=torch.Generator().manual_seed(52))) if per_pixel else None
     cost, lowest, planes_bd, mask, used = emu.mlp_forward(t, D, wts, planes=planes)
-    assert used == "mlp_tc_tcgen05_f16x3"
+    assert used == "mlp_tc_wgmma_f16x3"
     oc, ol, op, om = O.forward_mlp(**t, weights=tuple(wts), num_depth_bins=D, depth_planes_bdhw=planes,
                                    return_mask=True)
-    assert_cost_close("mlp", cost, oc, what="emu tcgen05")
-    assert_lowest_close("mlp", lowest, planes if per_pixel else planes_bd.view(B, D, 1, 1), oc, what="emu tcgen05")
-    assert_mask_close(mask, om, what="emu tcgen05")
+    assert_cost_close("mlp", cost, oc, what="emu wgmma")
+    assert_lowest_close("mlp", lowest, planes if per_pixel else planes_bd.view(B, D, 1, 1), oc, what="emu wgmma")
+    assert_mask_close(mask, om, what="emu wgmma")
     # the fp32 SIMT variant of the same call agrees to the split's 2^-21
     lib.srcv_set_variant(N.VARIANT_GENERIC)
     cost_g, *_ = emu.mlp_forward(t, D, wts, planes=planes)
@@ -277,8 +278,8 @@ def test_dot_forward_compile_time_map_size(lib):
 
 
 @pytest.mark.skipif(not __import__("os").environ.get("SRCV_EMU_SLOW"), reason="several minutes: set SRCV_EMU_SLOW=1")
-def test_mlp_forward_tcgen05_compile_time_map_size(lib):
-    """The 160x120 instantiation of the tcgen05 kernel on one full-size frame, one plane chunk
+def test_mlp_forward_wgmma_compile_time_map_size(lib):
+    """The 160x120 instantiation of the wgmma kernel on one full-size frame, one plane chunk
     (600 tiles through the 640-thread pipeline)."""
     lib.emu_set_sms(8)
     lib.srcv_set_variant(N.VARIANT_AUTO)
@@ -286,13 +287,13 @@ def test_mlp_forward_tcgen05_compile_time_map_size(lib):
     t = make_tuple(B, K, H, W, channels=C_, seed=92)
     wts = _weights(K, C_)
     cost, lowest, planes_bd, mask, used = emu.mlp_forward(t, D, wts)
-    assert used == "mlp_tc_tcgen05_f16x3"
+    assert used == "mlp_tc_wgmma_f16x3"
     oc, ol, op, om = O.forward_mlp(**t, weights=tuple(wts), num_depth_bins=D, return_mask=True)
     o64, *_ = O.forward_mlp(**{k: v.double() for k, v in t.items()}, weights=tuple(w.double() for w in wts),
                             num_depth_bins=D)
     # at 160-pixel coordinates the reference's own fp32 run is ~1.5e-5 off its fp64 evaluation
-    assert_cost_close("mlp", cost, oc, o64, what="emu tcgen05 160x120")
-    assert_mask_close(mask, om, what="emu tcgen05 160x120")
+    assert_cost_close("mlp", cost, oc, o64, what="emu wgmma 160x120")
+    assert_mask_close(mask, om, what="emu wgmma 160x120")
 
 
 def test_forward_sweeps_are_deterministic(lib):
@@ -309,7 +310,7 @@ def test_forward_sweeps_are_deterministic(lib):
     wts = _weights(7, 16)
     a = emu.mlp_forward(t, 8, wts)
     b = emu.mlp_forward(t, 8, wts)
-    assert a[4] == "mlp_tc_tcgen05_f16x3"
+    assert a[4] == "mlp_tc_wgmma_f16x3"
     assert torch.equal(a[0], b[0]) and torch.equal(a[1], b[1]) and torch.equal(a[3], b[3])
 
 

@@ -16,7 +16,7 @@ import simplerecon_b200 as S
 from oracle import costvolume_oracle as O
 from simplerecon_b200 import _native, cost_volume
 from simplerecon_b200.synthetic import make_tuple, mlp_state
-from tests import emu
+from tests import emu, refgolden
 from tests.parity import assert_cost_close, assert_lowest_close, assert_mask_close
 
 
@@ -229,14 +229,33 @@ def test_per_frame_depth_range_and_weight_image_cache(emulated):
     wts = O.mlp_weights_from_state_dict(m.state_dict())
     oc, ol, op, _ = O.forward_mlp(**t, weights=wts, num_depth_bins=D)
     assert torch.allclose(planes, op, rtol=3e-7, atol=0)
-    assert_cost_close("mlp", cost3, oc, what="per-frame range, tcgen05/emu")
+    assert_cost_close("mlp", cost3, oc, what="per-frame range, wgmma/emu")
+
+
+FAST_WARP_CASE = (2, 3, 8, 9, 12, 4)
+
+
+def reference_outputs():
+    """The reference FastFeatureVolumeManager.warp_features on the inputs of the test below
+    (tests/golden/make_reference_golden.py)."""
+    from oracle.ref_import import load_reference
+    R = load_reference()
+    B, K, C, H, W, D = FAST_WARP_CASE
+    t = make_tuple(B, K, H, W, channels=C, seed=31)
+    planes = _hero(K, C, H, W, D, fast=True).generate_depth_planes(B, t["min_depth"], t["max_depth"])
+    ref = R.FastFeatureVolumeManager(H, W, num_depth_bins=D)
+    uv_scale = torch.tensor([1.0 / W, 1.0 / H]).view(1, 1, 1, 2)
+    with torch.no_grad():
+        rw, rd, rf, rm, rp = ref.warp_features(t["src_feats"], t["src_extrinsics"], t["src_Ks"], t["cur_invK"],
+                                               planes, B, K, C, uv_scale)
+    return {"fast_warp": dict(world=rw, depths=rd, warped=rf, mask=rm, pix=rp)}
 
 
 def test_fast_manager_warp_features_five_tuple(emulated):
     """FastFeatureVolumeManager.warp_features (reference modules/cost_volume.py:812-964): all planes
     at once, 5-tuple (world points, depths, warped, mask, pixel coordinates) — against the oracle,
-    and against the live reference class where /root/reference is mounted."""
-    B, K, C, H, W, D = 2, 3, 8, 9, 12, 4
+    and against the stored outputs of the unmodified reference class (tests/refgolden.py)."""
+    B, K, C, H, W, D = FAST_WARP_CASE
     t = make_tuple(B, K, H, W, channels=C, seed=31)
     m = _hero(K, C, H, W, D, fast=True)
     planes = m.generate_depth_planes(B, t["min_depth"], t["max_depth"])
@@ -255,17 +274,11 @@ def test_fast_manager_warp_features_five_tuple(emulated):
         assert torch.allclose(pix[:, :, d, 1].reshape(B, K, -1), py, rtol=0, atol=2e-4)
         assert torch.equal(mask[:, :, d].reshape(B, K, -1), (zp > 0).float())
         assert torch.allclose(world[:, 0, d, :3].reshape(B, 3, -1), X, rtol=1e-6, atol=1e-7)
-    from oracle.ref_import import load_reference, reference_available
-    if reference_available():
-        R = load_reference()
-        ref = R.FastFeatureVolumeManager(H, W, num_depth_bins=D)
-        uv_scale = torch.tensor([1.0 / W, 1.0 / H]).view(1, 1, 1, 2)
-        with torch.no_grad():
-            rw, rd, rf, rm, rp = ref.warp_features(t["src_feats"], t["src_extrinsics"], t["src_Ks"], t["cur_invK"],
-                                                   planes, B, K, C, uv_scale)
-        assert torch.allclose(world, rw, rtol=1e-6, atol=1e-7) and torch.equal(mask, rm)
-        assert torch.allclose(depths, rd, rtol=2e-6, atol=1e-6) and torch.allclose(pix, rp, rtol=0, atol=2e-4)
-        assert (warped - rf).abs().max().item() <= 4e-5 * rf.abs().max().item() + 1e-6
+    G = refgolden.load("emu_python_stack", "fast_warp")
+    rw, rd, rf, rm, rp = G["world"], G["depths"], G["warped"], G["mask"], G["pix"]
+    assert torch.allclose(world, rw, rtol=1e-6, atol=1e-7) and torch.equal(mask, rm)
+    assert torch.allclose(depths, rd, rtol=2e-6, atol=1e-6) and torch.allclose(pix, rp, rtol=0, atol=2e-4)
+    assert (warped - rf).abs().max().item() <= 4e-5 * rf.abs().max().item() + 1e-6
 
 
 def test_producer_side_fusion_chunk_planar_and_raw_poses(emulated):

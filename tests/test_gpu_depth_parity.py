@@ -1,7 +1,7 @@
 """GPU half of the depth-map parity check (BASELINE target: depth Abs-Diff <= 1e-4 through the
 reference's U-Net): our cost volumes for a batch of seeded 640x480 tuples — 8 hero frames in one
-B = 8 call, 4 dot frames — written to gpurun_out/depth_parity_ours.npz.  The reference's decoder
-exists only in the build container, so the evaluation is tests/test_depth_parity_eval.py there
+B = 8 call, 4 dot frames — written to scripts/depth_parity.py's DUMP.  The reference's decoder
+exists only in the SimpleRecon source tree, so the evaluation is tests/test_depth_parity_eval.py there
 (scripts/depth_parity.py holds both halves)."""
 import importlib.util
 from pathlib import Path
@@ -21,4 +21,4 @@ def test_dump_cost_volumes_for_depth_parity(cuda_device):
     z = np.load(dp.DUMP)
     assert z["hero_cost"].shape == (8, 64, 120, 160) and z["dot_cost"].shape == (4, 64, 120, 160)
     assert np.isfinite(z["hero_cost"]).all() and np.isfinite(z["dot_cost"]).all()
-    assert "tcgen05" in str(z["hero_variant"]) and "fast" in str(z["dot_variant"])
+    assert "wgmma" in str(z["hero_variant"]) and "fast" in str(z["dot_variant"])

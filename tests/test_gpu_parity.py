@@ -1,4 +1,4 @@
-"""GPU parity: the sm_100a kernels (through the C ABI, via the manager classes)
+"""GPU parity: the sm_90a kernels (through the C ABI, via the manager classes)
 against (1) the committed golden vectors of the unmodified reference, (2) the CPU
 oracle on seeded inputs, (3) size-independent properties at BASELINE.json's full
 sizes.  Tolerances are stated in tests/parity.py."""
@@ -48,7 +48,7 @@ def fast_ok(kind, inputs):
     B, K, C, H, W = inputs["src_feats"].shape
     if kind == "dot":
         return C == 16                      # chunk-planar gather kernel
-    return C == 16 and K == 7               # tcgen05 kernel: hero layout (hidden widths 128/128)
+    return C == 16 and K == 7               # wgmma kernel: hero layout (hidden widths 128/128)
 
 
 # --------------------------------------------------------------------------- #
@@ -60,7 +60,10 @@ def test_golden(name, variant):
     g, inputs, sd = load_golden(name)
     kind = g["kind"]
     if variant == "fast" and not fast_ok(kind, inputs):
-        pytest.skip("fast variant does not cover this shape")
+        # forcing a variant on a shape it does not cover is an error, never a silent fallback
+        with pytest.raises(_native.SrcvError, match="variant needs"):
+            run_gpu(kind, inputs, g["D"], sd, variant)
+        return
     (cost, lowest, planes, mask), used = run_gpu(kind, inputs, g["D"], sd, variant)
     assert (("fast" in used) or ("tc" in used)) == (variant == "fast"), used
     assert cost.is_contiguous() and cost.dtype == torch.float32 and cost.is_cuda
@@ -82,7 +85,7 @@ def test_golden(name, variant):
 @pytest.mark.parametrize("name", golden_fullsize_names())
 def test_golden_full_size(name, variant):
     """The unmodified reference's outputs at the bench feature-map size (120 x 160, 7 views): the fast
-    variants run their compile-time 160 x 120 instantiations here (the dot sweep and the tcgen05 kernel)."""
+    variants run their compile-time 160 x 120 instantiations here (the dot sweep and the wgmma kernel)."""
     g, inputs, sd = load_golden_fullsize(name)
     kind = g["kind"]
     (cost, lowest, planes, mask), used = run_gpu(kind, inputs, g["D"], sd, variant)
@@ -123,9 +126,12 @@ def test_dot_vs_oracle(B, K, H, W, D, seed, smooth, variant):
 ])
 def test_mlp_vs_oracle(B, K, C, H, W, D, seed, variant):
     t = make_tuple(B, K, H, W, channels=C, seed=seed)
-    if variant == "fast" and not fast_ok("mlp", t):
-        pytest.skip("tensor-core variant covers the hero layout only")
     sd = mlp_state(K, C, seed=seed)
+    if variant == "fast" and not fast_ok("mlp", t):
+        # the tensor-core variant covers the hero layout only; forcing it elsewhere is an error
+        with pytest.raises(_native.SrcvError, match="tensor-core MLP variant needs"):
+            run_gpu("mlp", t, D, sd, variant)
+        return
     (cost, lowest, planes, mask), used = run_gpu("mlp", t, D, sd, variant)
     assert ("tc" in used) == (variant == "fast"), used
     w = O.mlp_weights_from_state_dict(sd)
@@ -354,7 +360,7 @@ def test_bench_gpu_arm_prints_one_json_line():
     assert d["n_gpus"] == 1 and d["steps"] == 10 and d["value"] > 0 and d["gpu_launches"] >= 20
     # default workload = hero model, 8 frames per GPU (BASELINE configs[2]; configs[4] at 8 GPUs)
     assert d["config"]["workload"].startswith("cfg2_hero") and d["config"]["batch_per_gpu"] == 8
-    assert d["dtype"] == "f32" and d["scaling"] == "weak" and "tcgen05" in d["kernel_variant"]
+    assert d["dtype"] == "f32" and d["scaling"] == "weak" and "wgmma" in d["kernel_variant"]
     rf = d["roofline"]
     assert rf["bound"] == "tensor" and 0 < rf["frac"] < 1.2 and rf["peak"] > 500 and rf["achieved"] > 0
     assert 0 < rf["hbm"]["frac"] < 1.5 and rf["issued_mma"]["achieved"] > 2.8 * rf["achieved"]

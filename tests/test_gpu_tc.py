@@ -1,7 +1,7 @@
-"""GPU: the tcgen05 building block on its own — D = A W^T through TMEM-resident A
-(fp16 hi/lo split), core-matrix weights in shared memory, three MMAs per K step —
-against an fp64 matmul.  Pins the TMEM packing order, the shared-memory descriptor,
-the instruction descriptor and the mbarrier protocol the metadata-MLP kernel uses."""
+"""GPU: the wgmma building block on its own — D = A W^T with A (fp16 hi/lo split) and the
+core-matrix weights in shared memory, three MMAs per K step — against an fp64 matmul.  Pins the
+core-matrix packing order, the shared-memory descriptors and the accumulator fragment layout the
+metadata-MLP kernel uses."""
 import ctypes as C
 
 import pytest
@@ -30,7 +30,7 @@ def test_tc_gemm_matches_fp64(cuda_device, built_lib, Kp, scale):
     e32 = (ref32 - ref).abs().max().item()
     # ... plus the fp16-subnormal floor of the lo halves (|x| < ~0.1 keeps an absolute 3e-8)
     bound = 4 * max(e32, 1e-7 * float(ref.abs().max())) + 6e-8 * 0.07 * Kp ** 0.5 * 2
-    assert err <= bound, f"tcgen05 GEMM err {err:.3e} (fp32 matmul err {e32:.3e})"
+    assert err <= bound, f"wgmma GEMM err {err:.3e} (fp32 matmul err {e32:.3e})"
 
 
 def test_tc_gemm_structured_operands(cuda_device, built_lib):

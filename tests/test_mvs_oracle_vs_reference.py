@@ -1,5 +1,6 @@
-"""CPU, build container only: the multi-view consistency oracle against the LIVE reference
-process_depth (tools/torch_point_cloud_fusion.py), whose hard-wired .cuda() calls are made no-ops."""
+"""CPU: the multi-view consistency oracle against the unmodified reference process_depth
+(tools/torch_point_cloud_fusion.py, its hard-wired .cuda() calls made no-ops when the stored outputs
+are generated; stored under tests/golden/reference/, see tests/refgolden.py)."""
 import importlib.util
 import os
 
@@ -8,13 +9,11 @@ import pytest
 import torch
 
 from oracle import mvs_oracle as M
-from oracle.ref_import import reference_available, reference_root
 from simplerecon_b200.synthetic import make_mvs_scene
-
-pytestmark = pytest.mark.skipif(not reference_available(), reason="reference tree not mounted")
-
+from tests import refgolden
 
 def _load_reference_fuser(monkeypatch):
+    from oracle.ref_import import reference_root
     import sys
     import types
     if "tqdm" not in sys.modules:
@@ -32,15 +31,41 @@ def _load_reference_fuser(monkeypatch):
     return mod
 
 
-@pytest.mark.parametrize("seed,n,hw", [(1, 5, (24, 32)), (2, 9, (30, 40))])
-def test_process_depth_matches_live_reference(monkeypatch, seed, n, hw):
-    R = _load_reference_fuser(monkeypatch)
+CASES = [(1, 5, (24, 32)), (2, 9, (30, 40))]
+
+
+def _ref_indices(n):
+    return (0, n // 2)
+
+
+def reference_outputs():
+    """For tests/golden/make_reference_golden.py."""
+    import _pytest.monkeypatch
+    mp = _pytest.monkeypatch.MonkeyPatch()
+    try:
+        R = _load_reference_fuser(mp)
+        out = {}
+        for seed, n, hw in CASES:
+            sc = make_mvs_scene(seed=seed, frames=n, height=hw[0], width=hw[1])
+            depths, images, P, K = sc["depths"], sc["images"], sc["cam_T_world"], sc["K"]
+            for ref_idx in _ref_indices(n):
+                src = torch.arange(n) != ref_idx
+                rp, rrgb, rvalid = R.process_depth(depths[ref_idx], images[ref_idx], depths[src], images[src],
+                                                   P[ref_idx], P[src], K[ref_idx], K[src], 0.1, 3)
+                out[f"{seed}_{n}_{ref_idx}"] = dict(points=np.asarray(rp), rgb=np.asarray(rrgb), valid=np.asarray(rvalid))
+        return out
+    finally:
+        mp.undo()
+
+
+@pytest.mark.parametrize("seed,n,hw", CASES)
+def test_process_depth_matches_live_reference(seed, n, hw):
     sc = make_mvs_scene(seed=seed, frames=n, height=hw[0], width=hw[1])
     depths, images, P, K = sc["depths"], sc["images"], sc["cam_T_world"], sc["K"]
-    for ref_idx in (0, n // 2):
+    for ref_idx in _ref_indices(n):
+        G = refgolden.load("mvs_oracle_vs_reference", f"{seed}_{n}_{ref_idx}")
+        rp, rrgb, rvalid = G["points"].numpy(), G["rgb"].numpy(), G["valid"].numpy()
         src = torch.arange(n) != ref_idx
-        rp, rrgb, rvalid = R.process_depth(depths[ref_idx], images[ref_idx], depths[src], images[src],
-                                           P[ref_idx], P[src], K[ref_idx], K[src], 0.1, 3)
         pts_avg, n_valid, valid = M.process_depth_dense(depths[ref_idx], depths[src], P[ref_idx], P[src],
                                                         K[ref_idx], K[src], 0.1, 3)
         assert np.array_equal(valid.numpy(), rvalid) and 0.05 < valid.float().mean().item() < 0.99

@@ -62,7 +62,7 @@ def _oracle_grads(t, wts, D, gcost, planes, dtype=torch.float64):
 
 
 @pytest.mark.parametrize("B,K,C,H,W,D,hidden,per_pixel,fast", [
-    (1, 7, 16, 16, 20, 4, (128, 128), False, False),   # hero layout: tcgen05 forward, fp32 recompute backward
+    (1, 7, 16, 16, 20, 4, (128, 128), False, False),   # hero layout: wgmma forward, fp32 recompute backward
     (2, 2, 8, 13, 17, 3, (128, 128), True, False),     # generic forward, per-pixel planes, ragged tiles
     (1, 3, 16, 12, 16, 5, (96, 64), False, True),      # narrow hidden layers, Fast manager class
 ])
