@@ -5,12 +5,14 @@
 // K = 7 source views, C = 16 channels, MLP 202 -> 128 -> 128 -> 1.
 //
 // One persistent CTA per SM walks over 64-row tiles (a 16 x 2 pixel patch at two consecutive planes):
-//   * 8 BUILDER warps (four threads per row, two K blocks each) project, gather, blend, build the
-//     metadata channels and write the row's fp16 (hi, lo) layer-1 operand into a 48 KB shared tile;
-//   * 2 CONSUMER warpgroups take tiles in turn: layer 1 = 12 x 3 wgmma m64n128k16 (A_hi W_hi + A_hi W_lo
-//     + A_lo W_hi), after which the tile goes back to the builders; the layer-1 accumulator fragment,
-//     biased, LeakyReLU'd and split in registers, IS the register A operand of layer 2 (8 x 3 wgmma
-//     m64n64k16 per 64-column half); the 128 -> 1 layer is a per-row dot product reduced over a quad.
+//   * 8 BUILDER warps (four threads per row, two K blocks = one 48-wide K chunk each) project, gather,
+//     blend, build the metadata channels and write the row's fp16 (hi, lo) layer-1 operand chunk by
+//     chunk into a 5-slot ring of 12 KB chunks;
+//   * 2 CONSUMER warpgroups take tiles in turn: layer 1 = 4 chunks x 3 x 3 wgmma m64n128k16 (A_hi W_hi
+//     + A_hi W_lo + A_lo W_hi), one commit group per chunk, each chunk's ring slot handed back as soon
+//     as its group retires; the layer-1 accumulator fragment, biased, LeakyReLU'd and split in
+//     registers, IS the register A operand of layer 2 (8 x 3 wgmma m64n64k16 per 64-column half); the
+//     128 -> 1 layer is a per-row dot product reduced over a quad.
 // Stages are chained by mbarriers; weights (160 KB, K-major no-swizzle core matrices) stay resident in
 // shared memory, pulled in once by the bulk-copy engine.
 //
@@ -34,7 +36,7 @@ namespace {
 using namespace tc;
 
 #ifndef SRCV_TC_REGS_BUILD
-#define SRCV_TC_REGS_BUILD 96
+#define SRCV_TC_REGS_BUILD 104
 #endif
 
 constexpr int kC = 16, kViews = 7;
@@ -70,14 +72,21 @@ constexpr uint32_t kOffW1Hi = 0, kOffW1Lo = kW1Bytes, kOffW2Hi = 2 * kW1Bytes,
 constexpr uint32_t kVecFloats = 3 * kN + 4;   // b2 | 0.505 w3 | 0.495 w3 | b3
 // image = [W1hi | W1lo | W2hi | W2lo | vec] exactly as it sits in shared memory
 constexpr uint32_t kImageBytes = kOffVec + kVecFloats * 4;
-// the layer-1 operand tile: hi | lo, each kRows x kK1 halves as K-major core matrices
-constexpr uint32_t kALoOff = kRows * kK1 * 2;
-constexpr uint32_t kOffA = (kImageBytes + 127) & ~127u;
-constexpr uint32_t kOffBar = kOffA + 2 * kALoOff;
-constexpr uint32_t kOffFlag = kOffBar + 8 * 8;                  // 8 mbarrier slots (5 used)
-constexpr uint32_t kSmemBytes = kOffFlag + kSlots * kRows;     // mask bits [builder slot][row]
+// The layer-1 operand is built and consumed in K chunks: builder slot s writes K chunk s of a tile
+// (its two K blocks, 48 K positions = 3 k-steps).  Chunk n of the CTA's chunk sequence (tile n / 4,
+// chunk n % 4) lives in ring slot n % kRing: hi | lo, each kRows x 48 halves as K-major core matrices.
+constexpr int kChunkSteps = kK1 / 16 / kSlots;                  // 3 k-steps per chunk
+constexpr int kRing = 5;                                        // 6 slots do not fit next to the image
+constexpr uint32_t kChunkLo = kRows * (kK1 / kSlots) * 2;       // 6 KB: offset of the lo half
+constexpr uint32_t kChunkBytes = 2 * kChunkLo;
+constexpr uint32_t kOffRing = (kImageBytes + 127) & ~127u;
+constexpr uint32_t kOffBar = kOffRing + kRing * kChunkBytes;
+constexpr uint32_t kOffFlag = kOffBar + 16 * 8;                 // 16 mbarrier slots (3 kRing + 1 used)
+static_assert(3 * kRing + 1 <= 16, "mbarrier slots: full[kRing], free[kRing][2], image");
+constexpr uint32_t kSmemBytes = kOffFlag + kRing * kRows;       // mask bits [ring slot][row]
+static_assert(kSlots * kChunkSteps * 16 == kK1 && kBlkCols * 2 * 2 == kK1 / kSlots, "one chunk = two K blocks");
 static_assert(kSmemBytes <= 227 * 1024, "shared-memory budget of one CTA");
-// operand strides: one 8-wide K chunk of the A tile / of a 128-row weight matrix
+// operand strides: one 8-wide K group of an A chunk / of a 128-row weight matrix
 constexpr uint32_t kALbo = kRows * 16, kWLbo = kN * 16, kSbo = 128;
 
 // K-major no-swizzle core-matrix offset (in halves) of element (n, k) of an N x Kp operand
@@ -165,16 +174,16 @@ tc_frame_bias_kernel(srcv_mlp_weights w, const ViewParams* __restrict__ views, f
   pb[(size_t)b * kN + n] = (float)((double)kWScale * (acc + (double)w.b1[n]));
 }
 
-// 12 packed columns of one K block -> the A tile in shared memory (hi and lo halves).  `a_row`
-// points at the row's first core-matrix line; column c (K 2c, 2c + 1) sits in K chunk c / 4, so a
-// block (12 columns, starting at a multiple of 4) is three 16-byte stores per half.
+// 12 packed columns of one K block -> its K chunk in the ring (hi and lo halves).  `a_row` points at
+// the row's first core-matrix line of the chunk; column c (K 2c, 2c + 1) sits in K group c / 4, so a
+// block (12 columns, starting at column 0 or 12 of the chunk) is three 16-byte stores per half.
 __device__ __forceinline__ void store_block(uint8_t* a_row, uint32_t col, const uint32_t (&hi)[kBlkCols],
                                             const uint32_t (&lo)[kBlkCols]) {
 #pragma unroll
   for (int i = 0; i < 3; ++i) {
     uint8_t* p = a_row + ((col >> 2) + (uint32_t)i) * kALbo;
     *reinterpret_cast<uint4*>(p) = uint4{hi[4 * i], hi[4 * i + 1], hi[4 * i + 2], hi[4 * i + 3]};
-    *reinterpret_cast<uint4*>(p + kALoOff) = uint4{lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]};
+    *reinterpret_cast<uint4*>(p + kChunkLo) = uint4{lo[4 * i], lo[4 * i + 1], lo[4 * i + 2], lo[4 * i + 3]};
   }
 }
 
@@ -396,13 +405,29 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
               unsigned num_tiles) {
   SRCV_DYNAMIC_SMEM_ALIGNED(uint8_t, smem, 1024);
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + kOffBar);
-  // Consumer warpgroup c takes the tiles it = c, c + 2, ...; each barrier below exists once per
-  // consumer, so that a waiter never sees a phase of the other warpgroup's tile.
-  uint64_t* bar_a1_full = bars + 0;   // [2] builders -> consumer c: the A tile is written   (256 arrivals)
-  uint64_t* bar_a1_free = bars + 2;   // [2] consumer c -> builders: its layer-1 MMAs are done (128 arrivals)
-  uint64_t* bar_img = bars + 4;       // weight image landed in shared memory (bulk copies)
-  uint8_t* sflag = smem + kOffFlag;
-  uint8_t* sa = smem + kOffA;
+  // Chunk n = kSlots * it + s (tile it, K chunk s) goes to ring slot n % kRing in use u = n / kRing.
+  //   full[slot]:       builder slot s has written chunk n (64 arrivals); completes once per use, the
+  //                     consumer of chunk n waits with parity u & 1;
+  //   free[slot][u & 1]: the MMAs that read chunk n have retired (128 arrivals); completes once every
+  //                     OTHER use, the builder of chunk n + kRing waits with parity (u >> 1) & 1.
+  // A parity wait is exact only while the barrier is neither two phases ahead of the waiter nor one
+  // phase behind it (then the wait would return at once, on an older phase).
+  //   * full: the consumer of chunk n has waited for chunk n - 1 (same tile) or finished its previous
+  //     tile (s = 0); either way builder slot (n - kRing) % kSlots, which builds in tile order, has
+  //     written chunk n - kRing, so full[slot] has completed use u - 1.  It cannot complete use u + 1
+  //     before chunk n is released, which follows this wait.
+  //   * free: the two consumer warpgroups release chunks out of order across a tile boundary (tile
+  //     it's last chunk retires at its wait_group 0, while the other warpgroup may already release
+  //     chunk 0 of tile it + 1), so one free barrier per slot could be one phase behind the builder of
+  //     chunk n + kRing.  With a barrier per use parity, being behind means chunk n - 2 kRing is not yet
+  //     released; but this builder saw chunk n - kRing + 1 released (its own previous chunk's wait),
+  //     and every release chain from that chunk passes through the release of chunk n - 2 kRing.
+  //     It cannot be two phases ahead: use u + 2 needs chunk n + kRing, which this builder writes.
+  uint64_t* bar_full = bars;              // [kRing]     builders -> consumer
+  uint64_t* bar_free = bars + kRing;      // [kRing][2]  consumer -> builders
+  uint64_t* bar_img = bars + 3 * kRing;   // weight image landed in shared memory (bulk copies)
+  uint8_t* sflag = smem + kOffFlag;   // mask bits of the rows of the chunk in ring slot r: [r][row]
+  uint8_t* ring = smem + kOffRing;
   const float* svec = reinterpret_cast<const float*>(smem + kOffVec);
 
   // The warp index goes through a shuffle broadcast so that ptxas knows the role branches are
@@ -417,9 +442,10 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
   // ---- one-time setup ----------------------------------------------------------------
   if (tid == 0) {
     mbar_init(bar_img, 1);
-    for (int c = 0; c < kConsumers; ++c) {
-      mbar_init(bar_a1_full + c, kBuilders);
-      mbar_init(bar_a1_free + c, 128);
+    for (int r = 0; r < kRing; ++r) {
+      mbar_init(bar_full + r, kBuilders / kSlots);
+      mbar_init(bar_free + 2 * r, 128);
+      mbar_init(bar_free + 2 * r + 1, 128);
     }
     mbar_fence_init();
   }
@@ -442,30 +468,34 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
 
   if (warp < kBuildWarps) {
     // =============================== builders ============================================
-    // Four threads per row (slot = warp / 2): views 2 slot, 2 slot + 1; slot 3 builds view 6 and the
-    // view-independent tail.  The first block of tile it is built before the wait for the operand
-    // tile, so its gathers overlap the layer-1 MMAs of tile it - 1.
+    // Four threads per row (slot = warp / 2): views 2 slot, 2 slot + 1, i.e. K chunk `slot`; slot 3
+    // builds view 6 and the view-independent tail.  The first block of a chunk is built before the
+    // wait for its ring slot, so its gathers overlap the MMAs that still read the slot.
     reg_dec<kRegsBuild>();
     const int row = (warp & 1) * 32 + lane, slot = warp >> 1;
     const Centre ctr(W, H);
     const int blk_first = 2 * slot;
     const bool masks = mask_out != nullptr;
-    uint8_t* a_row = sa + (uint32_t)(row >> 3) * kSbo + (uint32_t)(row & 7) * 16u;
+    uint8_t* a_row = ring + (uint32_t)(row >> 3) * kSbo + (uint32_t)(row & 7) * 16u;
     RowCtx rc;
     uint32_t hi[kBlkCols], lo[kBlkCols];
     for (unsigned it = 0; it < n_local; ++it) {
       make_row<PER_PIXEL>(tile_id(it), row, W, H, HW, D, nd, tiles_x, tiles_xy, ctr, cur4g, frames, planes, rc);
       const bool wb = masks && rc.last_plane;
       unsigned bits = build_block<TW, HWC>(rc, blk_first, src4, views, W, H, HW, ctr, wb, hi, lo);
-      if (it > 0) mbar_wait(bar_a1_free + ((it - 1) & 1u), ((it - 1) >> 1) & 1u);   // tile it - 1 is out of it
-      store_block(a_row, (uint32_t)(kBlkCols * blk_first), hi, lo);
+      const unsigned n = kSlots * it + (unsigned)slot, rs = n % kRing;
+      if (n >= (unsigned)kRing) {                  // chunk n - kRing is out of the slot
+        const unsigned v = n / kRing - 1u;
+        mbar_wait(bar_free + 2 * rs + (v & 1u), (v >> 1) & 1u);
+      }
+      uint8_t* a_chunk = a_row + rs * kChunkBytes;
+      store_block(a_chunk, 0u, hi, lo);
       bits |= build_block<TW, HWC>(rc, blk_first + 1, src4, views, W, H, HW, ctr, wb, hi, lo);
-      store_block(a_row, (uint32_t)(kBlkCols * (blk_first + 1)), hi, lo);
-      // the consumer of tile it reads the mask bits before it frees the operand tile, and the next
-      // store into this slot follows this thread's wait on exactly that arrival
-      if (wb) sflag[slot * kRows + row] = (uint8_t)bits;
+      store_block(a_chunk, (uint32_t)kBlkCols, hi, lo);
+      // the consumer reads the chunk's mask bits before it frees the ring slot
+      sflag[rs * kRows + row] = (uint8_t)bits;
       fence_proxy_async_smem();                    // generic-proxy stores -> visible to wgmma
-      mbar_arrive(bar_a1_full + (it & 1u));
+      mbar_arrive(bar_full + rs);
     }
   } else {
     // =============================== consumers ===========================================
@@ -474,36 +504,48 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
     const int g = lane >> 2, q = lane & 3;
     const int r0 = 16 * wl + g, r1 = r0 + 8;       // the two tile rows of this thread's fragments
     const bool masks = mask_out != nullptr;
+    // Descriptors differ between k-steps only in the start-address field (address >> 4, far from
+    // overflowing into the LBO field), so each one is a base descriptor + an immediate.
     const uint32_t sbase = smem_u32(smem);
-    for (unsigned k = 0, it = (unsigned)c; it < n_local; ++k, it += kConsumers) {
-      const unsigned id = tile_id(it);
-      const int b = (int)(nd.div(id) / tiles_xy);
-      const RowOut o0 = row_out(id, r0, W, H, HW, D, nd, tiles_x, tiles_xy);
-      const RowOut o1 = row_out(id, r1, W, H, HW, D, nd, tiles_x, tiles_xy);
-      mbar_wait(bar_a1_full + c, k & 1u);
+    const uint64_t desc_ring = smem_desc(sbase + kOffRing, kALbo, kSbo);
+    const uint64_t desc_w1 = smem_desc(sbase + kOffW1Hi, kWLbo, kSbo);
+    const uint64_t desc_w2 = smem_desc(sbase + kOffW2Hi, kWLbo, kSbo);
+    auto release = [&](unsigned n) { mbar_arrive(bar_free + 2 * (n % kRing) + ((n / kRing) & 1u)); };
+    for (unsigned it = (unsigned)c; it < n_local; it += kConsumers) {
+      // ---- layer 1: D1 = 16 (W1 x) over 12 k-steps, three products each, one commit group per
+      // K chunk; a chunk's ring slot is released as soon as the group that reads it has retired
+      float d1[64];
       unsigned bits0 = 0, bits1 = 0;
-      if (masks && q == 0) {
+      wgmma_fence();
 #pragma unroll
-        for (int sl = 0; sl < kSlots; ++sl) {
-          if (o0.last_plane) bits0 |= sflag[sl * kRows + r0];
-          if (o1.last_plane) bits1 |= sflag[sl * kRows + r1];
+      for (int ch = 0; ch < kSlots; ++ch) {
+        const unsigned n = kSlots * it + (unsigned)ch, rs = n % kRing;
+        mbar_wait(bar_full + rs, (n / kRing) & 1u);
+        if (masks) {
+          bits0 |= sflag[rs * kRows + r0];
+          bits1 |= sflag[rs * kRows + r1];
+        }
+        const uint64_t da = desc_ring + rs * (kChunkBytes >> 4);
+#pragma unroll
+        for (int i = 0; i < kChunkSteps; ++i) {
+          const int ks = kChunkSteps * ch + i;
+          const uint64_t ahi = da + ((uint32_t)i * 2 * kALbo >> 4), alo = ahi + (kChunkLo >> 4);
+          const uint64_t bhi = desc_w1 + ((uint32_t)ks * 2 * kWLbo >> 4), blo = bhi + (kW1Bytes >> 4);
+          wgmma_ss_n128(d1, ahi, bhi, ks > 0 ? 1u : 0u);
+          wgmma_ss_n128(d1, ahi, blo, 1u);
+          wgmma_ss_n128(d1, alo, bhi, 1u);
+        }
+        wgmma_commit();
+        if (ch > 0) {
+          wgmma_wait<1>();                         // the previous chunk's group has retired
+          release(n - 1u);
         }
       }
-      // ---- layer 1: D1 = 16 (W1 x) over 12 k-steps, three products each
-      float d1[64];
-      wgmma_fence();
-#pragma unroll 1
-      for (int ks = 0; ks < kK1 / 16; ++ks) {
-        const uint32_t ahi = sbase + kOffA + (uint32_t)ks * 2 * kALbo;
-        const uint32_t bhi = sbase + kOffW1Hi + (uint32_t)ks * 2 * kWLbo, blo = bhi + kW1Bytes;
-        wgmma_ss_n128(d1, smem_desc(ahi, kALbo, kSbo), smem_desc(bhi, kWLbo, kSbo), ks > 0 ? 1u : 0u);
-        wgmma_ss_n128(d1, smem_desc(ahi, kALbo, kSbo), smem_desc(blo, kWLbo, kSbo), 1u);
-        wgmma_ss_n128(d1, smem_desc(ahi + kALoOff, kALbo, kSbo), smem_desc(bhi, kWLbo, kSbo), 1u);
-      }
-      wgmma_commit();
       wgmma_wait<0>();
       fence_regs(d1);
-      mbar_arrive(bar_a1_free + c);                // the builders may write tile it + 1
+      release(kSlots * it + kSlots - 1u);
+      const unsigned id = tile_id(it);
+      const int b = (int)(nd.div(id) / tiles_xy);
       // ---- layer-1 epilogue: + frame bias, LeakyReLU, (hi, lo) split into the layer-2 A fragments
       uint32_t a2hi[kK2 / 16][4], a2lo[kK2 / 16][4];
       const float* pb = frame_bias + (size_t)b * kN + 2 * q;
@@ -523,12 +565,13 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
         float d2[32];
         wgmma_fence();
 #pragma unroll
+        const uint64_t dh = desc_w2 + ((uint32_t)nh * (kN / 2) * 16 >> 4);
+#pragma unroll
         for (int ks = 0; ks < kK2 / 16; ++ks) {
-          const uint32_t bhi = sbase + kOffW2Hi + (uint32_t)nh * (kN / 2) * 16 + (uint32_t)ks * 2 * kWLbo;
-          const uint32_t blo = bhi + kW2Bytes;
-          wgmma_rs_n64(d2, a2hi[ks], smem_desc(bhi, kWLbo, kSbo), ks > 0 ? 1u : 0u);
-          wgmma_rs_n64(d2, a2hi[ks], smem_desc(blo, kWLbo, kSbo), 1u);
-          wgmma_rs_n64(d2, a2lo[ks], smem_desc(bhi, kWLbo, kSbo), 1u);
+          const uint64_t bhi = dh + ((uint32_t)ks * 2 * kWLbo >> 4), blo = bhi + (kW2Bytes >> 4);
+          wgmma_rs_n64(d2, a2hi[ks], bhi, ks > 0 ? 1u : 0u);
+          wgmma_rs_n64(d2, a2hi[ks], blo, 1u);
+          wgmma_rs_n64(d2, a2lo[ks], bhi, 1u);
         }
         wgmma_commit();
         wgmma_wait<0>();
@@ -536,11 +579,14 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
           const int n = nh * (kN / 2) + 8 * j + 2 * q;
+          // columns n, n + 1 of b2 | 0.505 w3 | 0.495 w3
+          const float2 b2 = *reinterpret_cast<const float2*>(svec + n);
+          const float2 wp = *reinterpret_cast<const float2*>(svec + kN + n);
+          const float2 wa = *reinterpret_cast<const float2*>(svec + 2 * kN + n);
 #pragma unroll
           for (int e = 0; e < 4; ++e) {
-            const int nn = n + (e & 1);
-            const float hv = fmaf(d2[4 * j + e], kUnscale2, svec[nn]);
-            const float t = fmaf(svec[2 * kN + nn], fabsf(hv), svec[kN + nn] * hv);
+            const float hv = fmaf(d2[4 * j + e], kUnscale2, (e & 1) ? b2.y : b2.x);
+            const float t = fmaf((e & 1) ? wa.y : wa.x, fabsf(hv), ((e & 1) ? wp.y : wp.x) * hv);
             if (e < 2) acc0 += t; else acc1 += t;
           }
         }
@@ -551,6 +597,9 @@ mlp_tc_kernel(srcv_shape s, const float4* __restrict__ cur4g, const float4* __re
       acc0 += __shfl_xor_sync(0xffffffffu, acc0, 2);
       acc1 += __shfl_xor_sync(0xffffffffu, acc1, 2);
       if (q == 0) {
+        // where the two rows go is recomputed here rather than held in registers across the MMAs
+        const RowOut o0 = row_out(id, r0, W, H, HW, D, nd, tiles_x, tiles_xy);
+        const RowOut o1 = row_out(id, r1, W, H, HW, D, nd, tiles_x, tiles_xy);
         const float b3 = svec[3 * kN];
         // overall mask of the LAST plane (reference :625-637): any view in front AND any view
         // inside the 2-pixel border, independently

@@ -14,7 +14,7 @@
 //     the packed accumulator words d[8 s .. 8 s + 7] of columns 16 s .. 16 s + 15 of an earlier layer.
 #pragma once
 #ifdef SRCV_HOST_EMU
-#include "emu_tc.h"   // tests/emu: functional host model of this layer (same names, same semantics)
+#include "emu_tc_async.h"   // tests/emu: functional host model of this layer (same names, same semantics)
 #else
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
