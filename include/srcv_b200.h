@@ -293,6 +293,47 @@ size_t srcv_tsdf_workspace_bytes(const srcv_tsdf_frames* frames);
 int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* volume, const srcv_tsdf_frames* frames,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- marching-cubes mesh extraction from the TSDF volume ------------------------------ *
+ * Replaces TSDF.to_mesh (reference tools/tsdf.py:125-157: host copy of the volume, clamp, and
+ * scikit-image's marching_cubes at level 0) on the GPU.  The mesh is defined precisely (DESIGN
+ * §4.10) rather than byte-matched to scikit-image:
+ *   - values are taken to fp32 and clamped to [-1, 1]; a corner is inside iff its value is < 0;
+ *   - one vertex per crossing edge, shared between cubes, ordered by owning voxel (the edge's
+ *     lower endpoint) in linear order, then axis x, y, z; index-space position a + t (b - a) with
+ *     t = (0 - v_a) / (v_b - v_a) in fp32;
+ *   - normals: central-difference gradients (one-sided at the border) interpolated with t and
+ *     normalised, pointing toward increasing values (free space); zero gradient -> zero normal;
+ *   - faces: cube by cube in linear order, then in the order of the generated table
+ *     (simplerecon_b200/csrc/srcv_mc_table.h, scripts/gen_mc_table.py); right-hand normals point
+ *     toward increasing values; a triangle with two bitwise-equal fp32 index-space vertex
+ *     positions is dropped (allow_degenerate=False); the surface is closed away from the border
+ *     and from exact zeros;
+ *   - single_mesh (this library's reading of the reference's export_single_mesh): a cube is
+ *     processed only if all 8 corners have weight > 0, and a vertex is emitted only if a processed
+ *     cube contains its edge;
+ *   - scale_to_world: world = origin + v * voxel_size in fp32.  The reference's origin is fp16, so
+ *     callers pass origin already rounded to fp16.
+ * Two calls with the same args and workspace: srcv_mesh_count writes V and F to the DEVICE int64
+ * counts[2] (2 launches) and keeps them in the workspace; after reading them the caller allocates
+ * verts (V,3) f32, normals (V,3) f32 (or NULL) and faces (F,3) int32 and calls srcv_mesh_extract
+ * (2 launches), which first reads the kept totals back (16 bytes, a stream synchronisation) and
+ * refuses V / F that differ from them.  V > 2^31 - 1 is refused (faces are int32).
+ * Workspace: 4 bytes per voxel plus 24 bytes per 256 voxels.  X, Y, Z >= 2, X <= 65535,
+ * Y * Z < 2^31.  Deterministic: no atomics, fixed-order scans.                              */
+typedef struct srcv_mesh_args {
+  const void* tsdf_values;   /* DEVICE (X,Y,Z) fp16 */
+  const void* tsdf_weights;  /* DEVICE (X,Y,Z) fp16, read only when single_mesh */
+  int32_t X, Y, Z;
+  float origin[3];           /* already fp16-rounded by the caller */
+  float voxel_size;
+  int32_t scale_to_world, single_mesh;
+} srcv_mesh_args;
+size_t srcv_mesh_workspace_bytes(const srcv_mesh_args* args);
+int32_t srcv_mesh_count(const srcv_mesh_args* args, int64_t* counts, void* workspace, size_t workspace_bytes,
+                        void* stream);
+int32_t srcv_mesh_extract(const srcv_mesh_args* args, float* verts, float* normals, int32_t* faces, int64_t V,
+                          int64_t F, void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py
  * :12-97), which pc_fusion.py:158 runs for every frame of a scan against all the others: for each

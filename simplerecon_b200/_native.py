@@ -66,6 +66,12 @@ class TsdfFrames(C.Structure):
                 ("H", C.c_int32), ("W", C.c_int32), ("min_depth", C.c_float), ("max_depth", C.c_float)]
 
 
+class MeshArgs(C.Structure):
+    _fields_ = [("tsdf_values", _fp), ("tsdf_weights", _fp), ("X", C.c_int32), ("Y", C.c_int32), ("Z", C.c_int32),
+                ("origin", C.c_float * 3), ("voxel_size", C.c_float), ("scale_to_world", C.c_int32),
+                ("single_mesh", C.c_int32)]
+
+
 class MvsScan(C.Structure):
     _fields_ = [("depths", _fp), ("K", _fp), ("K_inv", _fp), ("cam_T_world", _fp), ("world_T_cam", _fp),
                 ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32)]
@@ -109,6 +115,9 @@ SYMBOLS = {
                                                       C.c_float, _fp, _fp, _fp]),
     "srcv_tsdf_workspace_bytes": (C.c_size_t, [C.POINTER(TsdfFrames)]),
     "srcv_tsdf_integrate_f16": (C.c_int32, [C.POINTER(TsdfVolume), C.POINTER(TsdfFrames), _fp, C.c_size_t, _fp]),
+    "srcv_mesh_workspace_bytes": (C.c_size_t, [C.POINTER(MeshArgs)]),
+    "srcv_mesh_count": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, C.c_size_t, _fp]),
+    "srcv_mesh_extract": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, _fp, C.c_int64, C.c_int64, _fp, C.c_size_t, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

@@ -455,6 +455,57 @@ int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frame
   return SRCV_OK;
 }
 
+static int32_t check_mesh(const srcv_mesh_args* a) {
+  if (!a) return fail(SRCV_ERR_NULL, "mesh arguments are NULL");
+  if (!a->tsdf_values) return fail(SRCV_ERR_NULL, "tsdf_values is NULL");
+  if (a->single_mesh && !a->tsdf_weights) return fail(SRCV_ERR_NULL, "single_mesh needs tsdf_weights");
+  if (a->X < 2 || a->Y < 2 || a->Z < 2)
+    return fail(SRCV_ERR_SHAPE, "bad volume dimensions %d x %d x %d (each must be >= 2)", a->X, a->Y, a->Z);
+  if (!mesh_shape_supported(*a))
+    return fail(SRCV_ERR_SHAPE, "volume %d x %d x %d out of range (X <= 65535, Y * Z < 2^31)", a->X, a->Y, a->Z);
+  if (a->scale_to_world && !(a->voxel_size > 0.f)) return fail(SRCV_ERR_SHAPE, "voxel_size must be positive");
+  if (((reinterpret_cast<uintptr_t>(a->tsdf_values) | reinterpret_cast<uintptr_t>(a->tsdf_weights)) & 1u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
+  return SRCV_OK;
+}
+
+size_t srcv_mesh_workspace_bytes(const srcv_mesh_args* a) {
+  if (!a || a->X < 2 || a->Y < 2 || a->Z < 2 || !mesh_shape_supported(*a)) return 0;
+  return mesh_workspace_bytes(*a);
+}
+
+int32_t srcv_mesh_count(const srcv_mesh_args* a, int64_t* counts, void* workspace, size_t workspace_bytes,
+                        void* stream_) {
+  if (int32_t e = check_mesh(a)) return e;
+  if (!counts) return fail(SRCV_ERR_NULL, "counts is NULL");
+  if (int32_t e = check_workspace(workspace, workspace_bytes, mesh_workspace_bytes(*a))) return e;
+  g_last_variant.store("tsdf_mesh_mc");
+  cudaError_t err = launch_mesh_count(*a, reinterpret_cast<long long*>(counts), workspace,
+                                      static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "mesh_count");
+  return SRCV_OK;
+}
+
+int32_t srcv_mesh_extract(const srcv_mesh_args* a, float* verts, float* normals, int32_t* faces, int64_t V,
+                          int64_t F, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_mesh(a)) return e;
+  if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
+  if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
+  if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
+  if (int32_t e = check_workspace(workspace, workspace_bytes, mesh_workspace_bytes(*a))) return e;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  long long totals[2] = {-1, -1};
+  cudaError_t err = mesh_read_totals(*a, workspace, totals, stream);
+  if (err != cudaSuccess) return cuda_fail(err, "mesh totals");
+  if (totals[0] != V || totals[1] != F)
+    return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match srcv_mesh_count (%lld, %lld) for this workspace",
+                (long long)V, (long long)F, totals[0], totals[1]);
+  g_last_variant.store("tsdf_mesh_mc");
+  err = launch_mesh_extract(*a, verts, normals, faces, workspace, stream);
+  if (err != cudaSuccess) return cuda_fail(err, "mesh_extract");
+  return SRCV_OK;
+}
+
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {
   if (!s || s->N <= 0) return 0;
   return mvs_workspace_bytes(s->N);

@@ -103,6 +103,14 @@ size_t tsdf_workspace_bytes(int frames);
 cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_frames& f, void* workspace,
                                   cudaStream_t stream);
 
+// marching-cubes mesh extraction from the TSDF volume (csrc/srcv_mesh.cuh)
+size_t mesh_workspace_bytes(const srcv_mesh_args& a);
+bool mesh_shape_supported(const srcv_mesh_args& a);
+cudaError_t launch_mesh_count(const srcv_mesh_args& a, long long* counts, void* workspace, cudaStream_t stream);
+cudaError_t mesh_read_totals(const srcv_mesh_args& a, void* workspace, long long totals[2], cudaStream_t stream);
+cudaError_t launch_mesh_extract(const srcv_mesh_args& a, float* verts, float* normals, int32_t* faces,
+                                void* workspace, cudaStream_t stream);
+
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);
 cudaError_t launch_mvs_consistency(const srcv_mvs_scan& s, int ref, float z_thresh, int n_consistent,

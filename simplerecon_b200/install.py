@@ -6,7 +6,10 @@
 binds the names at import time — reference experiment_modules/depth_model.py:10-11)
 so ``DepthModel`` builds the sm_90a-backed classes without any edit to the
 reference.  ``install(losses=True)`` also swaps the reference's ``losses.MVDepthLoss`` (the
-training loss of depth_model.py:144, :477-485) for the kernel-backed mirror.  See INTEGRATION.md.
+training loss of depth_model.py:144, :477-485) for the kernel-backed mirror.  ``install(fusion=True)``
+swaps ``tools.tsdf.TSDF`` / ``TSDFFuser`` for the kernel-backed mirrors (fusion and mesh export), and
+the names ``tools.fusers_helper`` bound at import (tools/fusers_helper.py:8) if it was already
+imported.  ``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
 
@@ -17,9 +20,10 @@ _NAMES = ("CostVolumeManager", "FeatureVolumeManager", "FastFeatureVolumeManager
 _saved: dict = {}
 
 
-def install(verbose: bool = False, losses: bool = False) -> list[str]:
+def install(verbose: bool = False, losses: bool = False, fusion: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
-    be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``."""
+    be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
+    with ``fusion=True`` also as ``tools.tsdf``."""
     from . import cost_volume as ours
     patched = []
     ref_cv = importlib.import_module("modules.cost_volume")
@@ -42,6 +46,17 @@ def install(verbose: bool = False, losses: bool = False) -> list[str]:
                 mod.MVDepthLoss = MVDepthLoss
                 if mod.__name__ not in patched:
                     patched.append(mod.__name__)
+    if fusion:
+        from . import tsdf as ours_tsdf
+        ref_tsdf = importlib.import_module("tools.tsdf")
+        fh = sys.modules.get("tools.fusers_helper")
+        for mod in [ref_tsdf] + ([fh] if fh is not None else []):
+            for n in ("TSDF", "TSDFFuser"):
+                if hasattr(mod, n):
+                    _saved.setdefault((mod.__name__, n), getattr(mod, n))
+                    setattr(mod, n, getattr(ours_tsdf, n))
+            if mod.__name__ not in patched:
+                patched.append(mod.__name__)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched
