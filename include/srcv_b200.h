@@ -293,6 +293,26 @@ size_t srcv_tsdf_workspace_bytes(const srcv_tsdf_frames* frames);
 int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* volume, const srcv_tsdf_frames* frames,
                                 void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- colour fusion into the TSDF volume (DESIGN §4.11) --------------------------------- *
+ * srcv_tsdf_integrate_color_f16 is srcv_tsdf_integrate_f16 (same volume, frames, workspace; values
+ * and weights bit-identical) that also averages each frame's colour into an fp32 colour volume:
+ *   colors   DEVICE (3,X,Y,Z) f32 R, G, B planes in [0, 1], z fastest, updated in place (0 = unseen)
+ *   images   DEVICE (B,3,Hc,Wc) f32, any Hc, Wc >= 1 (normalised with mean / std per channel)
+ * For every (voxel, frame) update of the values: the depth pixel (sx, sy) the update sampled maps to
+ * colour pixel (min(floor(sx * (Wc/W)), Wc-1), min(floor(sy * (Hc/H)), Hc-1)) (PyTorch's `nearest`,
+ * each scale an fp32 in/out), rgb = clamp((x - mean) / std, 0, 1), and
+ * c = (c * tw + rgb * nw) / total with the update's own fp16 old weight tw, nw and total, every op a
+ * separately rounded fp32 op.  The vector path also needs `colors` 16-byte aligned.              */
+typedef struct srcv_tsdf_color {
+  void* colors;
+  const void* images;
+  int32_t Hc, Wc;
+  float mean[3], std[3];
+} srcv_tsdf_color;
+int32_t srcv_tsdf_integrate_color_f16(const srcv_tsdf_volume* volume, const srcv_tsdf_frames* frames,
+                                      const srcv_tsdf_color* color, void* workspace, size_t workspace_bytes,
+                                      void* stream);
+
 /* ---- marching-cubes mesh extraction from the TSDF volume ------------------------------ *
  * Replaces TSDF.to_mesh (reference tools/tsdf.py:125-157: host copy of the volume, clamp, and
  * scikit-image's marching_cubes at level 0) on the GPU.  The mesh is defined precisely (DESIGN
@@ -333,6 +353,14 @@ int32_t srcv_mesh_count(const srcv_mesh_args* args, int64_t* counts, void* works
                         void* stream);
 int32_t srcv_mesh_extract(const srcv_mesh_args* args, float* verts, float* normals, int32_t* faces, int64_t V,
                           int64_t F, void* workspace, size_t workspace_bytes, void* stream);
+/* srcv_mesh_extract with vertex colours (DESIGN §4.11), after the same srcv_mesh_count and with the
+ * same workspace; verts, normals and faces are bitwise srcv_mesh_extract's.  colors is the DEVICE
+ * (3,X,Y,Z) f32 colour volume, args->tsdf_weights is required, vert_colors is (V,3) f32: each vertex
+ * takes the colour of its crossing edge (a, b) with the position's t — both endpoints weighted:
+ * ca + t (cb - ca) in fp32; one: that endpoint's colour; none: grey 0.7.                         */
+int32_t srcv_mesh_extract_color(const srcv_mesh_args* args, const void* colors, float* verts, float* normals,
+                                float* vert_colors, int32_t* faces, int64_t V, int64_t F, void* workspace,
+                                size_t workspace_bytes, void* stream);
 
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py

@@ -20,5 +20,6 @@ __all__ = [
 ]
 __version__ = "0.1.0"
 from .tsdf import TSDF, TSDFFuser  # noqa: E402,F401  (reference tools/tsdf.py)
+from .fusers import ColorFuser  # noqa: E402,F401  (OurFuser with colour, DESIGN §4.11)
 from . import point_cloud_fusion  # noqa: E402,F401  (reference tools/torch_point_cloud_fusion.py)
 from .losses import MVDepthLoss  # noqa: E402,F401  (reference losses.py:79-208)

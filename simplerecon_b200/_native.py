@@ -66,6 +66,11 @@ class TsdfFrames(C.Structure):
                 ("H", C.c_int32), ("W", C.c_int32), ("min_depth", C.c_float), ("max_depth", C.c_float)]
 
 
+class TsdfColor(C.Structure):
+    _fields_ = [("colors", _fp), ("images", _fp), ("Hc", C.c_int32), ("Wc", C.c_int32), ("mean", C.c_float * 3),
+                ("std", C.c_float * 3)]
+
+
 class MeshArgs(C.Structure):
     _fields_ = [("tsdf_values", _fp), ("tsdf_weights", _fp), ("X", C.c_int32), ("Y", C.c_int32), ("Z", C.c_int32),
                 ("origin", C.c_float * 3), ("voxel_size", C.c_float), ("scale_to_world", C.c_int32),
@@ -115,9 +120,13 @@ SYMBOLS = {
                                                       C.c_float, _fp, _fp, _fp]),
     "srcv_tsdf_workspace_bytes": (C.c_size_t, [C.POINTER(TsdfFrames)]),
     "srcv_tsdf_integrate_f16": (C.c_int32, [C.POINTER(TsdfVolume), C.POINTER(TsdfFrames), _fp, C.c_size_t, _fp]),
+    "srcv_tsdf_integrate_color_f16": (C.c_int32, [C.POINTER(TsdfVolume), C.POINTER(TsdfFrames), C.POINTER(TsdfColor),
+                                                  _fp, C.c_size_t, _fp]),
     "srcv_mesh_workspace_bytes": (C.c_size_t, [C.POINTER(MeshArgs)]),
     "srcv_mesh_count": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, C.c_size_t, _fp]),
     "srcv_mesh_extract": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, _fp, C.c_int64, C.c_int64, _fp, C.c_size_t, _fp]),
+    "srcv_mesh_extract_color": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int64, _fp,
+                                            C.c_size_t, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

@@ -433,8 +433,8 @@ size_t srcv_tsdf_workspace_bytes(const srcv_tsdf_frames* f) {
   return tsdf_workspace_bytes(f->B);
 }
 
-int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, void* workspace,
-                                size_t workspace_bytes, void* stream_) {
+static int32_t check_tsdf(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, void* workspace,
+                          size_t workspace_bytes) {
   if (!v || !f) return fail(SRCV_ERR_NULL, "volume / frames descriptor is NULL");
   if (!v->tsdf_values || !v->tsdf_weights) return fail(SRCV_ERR_NULL, "tsdf_values / tsdf_weights is NULL");
   if (!f->depth || !f->cam_T_world || !f->K) return fail(SRCV_ERR_NULL, "depth / cam_T_world / K is NULL");
@@ -449,9 +449,32 @@ int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frame
         reinterpret_cast<uintptr_t>(f->K)) & 1u) != 0)
     return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
   if (int32_t e = check_workspace(workspace, workspace_bytes, tsdf_workspace_bytes(f->B))) return e;
+  return SRCV_OK;
+}
+
+int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, void* workspace,
+                                size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_tsdf(v, f, workspace, workspace_bytes)) return e;
   g_last_variant.store("tsdf_integrate_f16");
   cudaError_t err = launch_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "tsdf_integrate");
+  return SRCV_OK;
+}
+
+int32_t srcv_tsdf_integrate_color_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, const srcv_tsdf_color* c,
+                                      void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!c) return fail(SRCV_ERR_NULL, "colour descriptor is NULL");
+  if (!c->colors || !c->images) return fail(SRCV_ERR_NULL, "colors / images is NULL");
+  if (int32_t e = check_tsdf(v, f, workspace, workspace_bytes)) return e;
+  if (c->Hc < 1 || c->Wc < 1 || (long long)c->Hc * c->Wc > (1ll << 30))
+    return fail(SRCV_ERR_SHAPE, "bad colour image size Hc=%d Wc=%d", c->Hc, c->Wc);
+  for (int ch = 0; ch < 3; ++ch)
+    if (!(c->std[ch] != 0.f)) return fail(SRCV_ERR_SHAPE, "colour std[%d] must be non-zero", ch);
+  if (((reinterpret_cast<uintptr_t>(c->colors) | reinterpret_cast<uintptr_t>(c->images)) & 3u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "f32 colour arrays must be 4-byte aligned");
+  g_last_variant.store("tsdf_integrate_color_f16");
+  cudaError_t err = launch_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_), c);
+  if (err != cudaSuccess) return cuda_fail(err, "tsdf_integrate_color");
   return SRCV_OK;
 }
 
@@ -486,9 +509,9 @@ int32_t srcv_mesh_count(const srcv_mesh_args* a, int64_t* counts, void* workspac
   return SRCV_OK;
 }
 
-int32_t srcv_mesh_extract(const srcv_mesh_args* a, float* verts, float* normals, int32_t* faces, int64_t V,
-                          int64_t F, void* workspace, size_t workspace_bytes, void* stream_) {
-  if (int32_t e = check_mesh(a)) return e;
+static int32_t mesh_extract(const srcv_mesh_args* a, const float* colors, float* verts, float* normals,
+                            float* vert_colors, int32_t* faces, int64_t V, int64_t F, void* workspace,
+                            size_t workspace_bytes, void* stream_) {
   if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
   if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
   if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
@@ -500,10 +523,28 @@ int32_t srcv_mesh_extract(const srcv_mesh_args* a, float* verts, float* normals,
   if (totals[0] != V || totals[1] != F)
     return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match srcv_mesh_count (%lld, %lld) for this workspace",
                 (long long)V, (long long)F, totals[0], totals[1]);
-  g_last_variant.store("tsdf_mesh_mc");
-  err = launch_mesh_extract(*a, verts, normals, faces, workspace, stream);
+  g_last_variant.store(colors ? "tsdf_mesh_mc_color" : "tsdf_mesh_mc");
+  err = launch_mesh_extract(*a, verts, normals, faces, workspace, stream, colors, vert_colors);
   if (err != cudaSuccess) return cuda_fail(err, "mesh_extract");
   return SRCV_OK;
+}
+
+int32_t srcv_mesh_extract(const srcv_mesh_args* a, float* verts, float* normals, int32_t* faces, int64_t V,
+                          int64_t F, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_mesh(a)) return e;
+  return mesh_extract(a, nullptr, verts, normals, nullptr, faces, V, F, workspace, workspace_bytes, stream_);
+}
+
+int32_t srcv_mesh_extract_color(const srcv_mesh_args* a, const void* colors, float* verts, float* normals,
+                                float* vert_colors, int32_t* faces, int64_t V, int64_t F, void* workspace,
+                                size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_mesh(a)) return e;
+  if (!a->tsdf_weights) return fail(SRCV_ERR_NULL, "vertex colours need tsdf_weights");
+  if (!colors) return fail(SRCV_ERR_NULL, "colors is NULL");
+  if (V > 0 && !vert_colors) return fail(SRCV_ERR_NULL, "vert_colors is NULL");
+  if ((reinterpret_cast<uintptr_t>(colors) & 3u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "colors must be 4-byte aligned");
+  return mesh_extract(a, static_cast<const float*>(colors), verts, normals, vert_colors, faces, V, F, workspace,
+                      workspace_bytes, stream_);
 }
 
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {

@@ -100,16 +100,19 @@ cudaError_t launch_instnorm_c4(const float* x, int B, int V, int C, int H, int W
 
 // dense-grid TSDF integration (csrc/srcv_tsdf.cu)
 size_t tsdf_workspace_bytes(int frames);
+// color != nullptr: also fuse the frames' colour into color->colors (DESIGN §4.11)
 cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_frames& f, void* workspace,
-                                  cudaStream_t stream);
+                                  cudaStream_t stream, const srcv_tsdf_color* color = nullptr);
 
 // marching-cubes mesh extraction from the TSDF volume (csrc/srcv_mesh.cuh)
 size_t mesh_workspace_bytes(const srcv_mesh_args& a);
 bool mesh_shape_supported(const srcv_mesh_args& a);
 cudaError_t launch_mesh_count(const srcv_mesh_args& a, long long* counts, void* workspace, cudaStream_t stream);
 cudaError_t mesh_read_totals(const srcv_mesh_args& a, void* workspace, long long totals[2], cudaStream_t stream);
+// colors != nullptr: also vertex colours (V,3) from the (3,X,Y,Z) colour volume (DESIGN §4.11)
 cudaError_t launch_mesh_extract(const srcv_mesh_args& a, float* verts, float* normals, int32_t* faces,
-                                void* workspace, cudaStream_t stream);
+                                void* workspace, cudaStream_t stream, const float* colors = nullptr,
+                                float* vert_colors = nullptr);
 
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);

@@ -382,6 +382,56 @@ mesh_vertex_kernel(MeshParams p, const int* __restrict__ block_counts, const lon
   }
 }
 
+// Vertex colours (DESIGN §4.11), a pass of its own after the vertex pass (same chunks, same vertex order):
+// each vertex takes the colour of its edge (a, b) from the (3,X,Y,Z) planes with the position's t.  Both
+// endpoints observed (weight > 0): ca + t (cb - ca); one: its colour; none: grey 0.7.  Separately rounded
+// fp32 ops.  (Folded into the vertex pass, the colour state lives across the normals' IEEE-division
+// slow-path calls and ptxas spills it.)
+template <int VEC>
+__global__ void __launch_bounds__(kMeshThreads)
+mesh_vertex_color_kernel(MeshParams p, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
+                         const float* __restrict__ colors, size_t cplane, float* __restrict__ vert_colors) {
+  if (block_counts[2 * block_linear()] == 0) return;    // the whole block owns no vertex (block-uniform)
+  const Chunk c = chunk_of<VEC>(p);
+  int nv, nf, ta, tb;
+  chunk_counts<VEC>(p, c, nv, nf);
+  nf = 0;
+  block_scan2(nv, nf, ta, tb);
+  if (!c.live) return;
+  long long off = block_off[2 * block_linear()] + nv;
+  for (int i = 0; i < VEC; ++i) {
+    const int x = c.x, y = c.y, z = c.z0 + i;
+    const unsigned m = owned_edges(p, x, y, z);
+    if (m == 0u) continue;
+    const size_t ia = vidx(p, x, y, z);
+    const float v0 = ld(p, x, y, z);
+    const bool oa = __half2float(p.w[ia]) > 0.0f;
+#pragma unroll
+    for (int a = 0; a < 3; ++a) {
+      if (!((m >> a) & 1u)) continue;
+      const int qx = x + (a == 0), qy = y + (a == 1), qz = z + (a == 2);
+      const size_t ib = vidx(p, qx, qy, qz);
+      const float t = edge_t(v0, ld(p, qx, qy, qz));           // the position's t (mesh_vertex_kernel)
+      const bool ob = __half2float(p.w[ib]) > 0.0f;
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        const float* cc = colors + ch * cplane;
+        float r = 0.7f;
+        if (oa && ob) {
+          const float ca = cc[ia];
+          r = __fadd_rn(ca, __fmul_rn(t, __fadd_rn(cc[ib], -ca)));
+        } else if (oa) {
+          r = cc[ia];
+        } else if (ob) {
+          r = cc[ib];
+        }
+        vert_colors[3 * off + ch] = r;
+      }
+      ++off;
+    }
+  }
+}
+
 template <int VEC>
 __global__ void __launch_bounds__(kMeshThreads)
 mesh_face_kernel(MeshParams p, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
@@ -506,7 +556,7 @@ cudaError_t mesh_read_totals(const srcv_mesh_args& a, void* workspace, long long
 }
 
 cudaError_t launch_mesh_extract(const srcv_mesh_args& a, float* verts, float* normals, int32_t* faces,
-                                void* workspace, cudaStream_t stream) {
+                                void* workspace, cudaStream_t stream, const float* colors, float* vert_colors) {
   const MeshWs w = carve(a, workspace);
   const int vec = vec_of(a);
   const MeshParams p = params(a, vec);
@@ -515,6 +565,14 @@ cudaError_t launch_mesh_extract(const srcv_mesh_args& a, float* verts, float* no
   note_launch();
   cudaError_t err = cudaGetLastError();
   if (err != cudaSuccess) return err;
+  if (colors != nullptr) {
+    const size_t cplane = (size_t)a.X * a.Y * a.Z;
+    if (vec == kMeshVec) SRCV_LAUNCH(mesh_vertex_color_kernel<kMeshVec>, grid_of(a, vec), kMeshThreads, 0, stream, p, w.block_counts, w.block_off, colors, cplane, vert_colors);
+    else SRCV_LAUNCH(mesh_vertex_color_kernel<1>, grid_of(a, vec), kMeshThreads, 0, stream, p, w.block_counts, w.block_off, colors, cplane, vert_colors);
+    note_launch();
+    err = cudaGetLastError();
+    if (err != cudaSuccess) return err;
+  }
   if (vec == kMeshVec) SRCV_LAUNCH(mesh_face_kernel<kMeshVec>, grid_of(a, vec), kMeshThreads, 0, stream, p, w.block_counts, w.block_off, w.vbase, faces);
   else SRCV_LAUNCH(mesh_face_kernel<1>, grid_of(a, vec), kMeshThreads, 0, stream, p, w.block_counts, w.block_off, w.vbase, faces);
   note_launch();

@@ -71,10 +71,22 @@ __global__ void tsdf_prep_kernel(const __half* __restrict__ K, const __half* __r
   frames[b].P[i * 4 + k] = r16(acc);
 }
 
-template <int VEC>
-__global__ void __launch_bounds__(256)
-tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
-                      const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights) {
+// Colour fusion (DESIGN §4.11): fp32 (3,X,Y,Z) R/G/B planes averaged with the value's own weights.
+struct TsdfColorParams {
+  float* colors;               // (3, X, Y, Z) planes, z fastest
+  const float* images;         // (B, 3, Hc, Wc) of this launch's frames, normalised
+  size_t plane;                // X * Y * Z
+  int Hc, Wc;
+  float scale_x, scale_y;      // Wc / W, Hc / H in fp32: PyTorch's `nearest` source-index scale
+  float mean[3], std[3];       // de-normalisation (x - mean) / std, then clamp to [0, 1]
+};
+
+// The kColor = false instantiation is the plain kernel: every colour statement is `if constexpr`.
+template <int VEC, bool kColor>
+__device__ __forceinline__ void
+tsdf_integrate_body(const TsdfParams& p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
+                    const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights,
+                    const TsdfColorParams& cp) {
   // grid.y walks x; grid.x * blockDim.x covers the (y, z-column) plane: 32-bit index arithmetic only
   // (64-bit div/mod of a flat voxel index cost more than the projection of an empty column)
   const unsigned zcols = (unsigned)(p.Z / VEC);
@@ -120,6 +132,7 @@ tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const 
   for (int i = 0; i < VEC; ++i) wz[i] = r16(__fadd_rn(p.oz, __fmul_rn((float)(z0 + i), p.voxel_size)));
 
   float tv[VEC], tw[VEC];
+  float tc[3][kColor ? VEC : 1];
   bool loaded = false, dirty = false;
 
   for (int b = 0; b < p.B; ++b) {
@@ -168,6 +181,20 @@ tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const 
 #pragma unroll
           for (int j = 0; j < VEC; ++j) { tv[j] = __half2float(tsdf[base + j]); tw[j] = __half2float(weights[base + j]); }
         }
+        if constexpr (kColor) {
+#pragma unroll
+          for (int ch = 0; ch < 3; ++ch) {
+            const float* src = cp.colors + ch * cp.plane + base;
+            if (VEC == 8) {
+              const float4 c0 = *reinterpret_cast<const float4*>(src), c1 = *reinterpret_cast<const float4*>(src + 4);
+              tc[ch][0] = c0.x; tc[ch][1] = c0.y; tc[ch][2] = c0.z; tc[ch][3] = c0.w;
+              tc[ch][4] = c1.x; tc[ch][5] = c1.y; tc[ch][6] = c1.z; tc[ch][7] = c1.w;
+            } else {
+#pragma unroll
+              for (int j = 0; j < VEC; ++j) tc[ch][j] = src[j];
+            }
+          }
+        }
         loaded = true;
       }
       // :307-318: running average with InfiniTAM's confidence-dependent rate
@@ -175,6 +202,19 @@ tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const 
       const float nw = r16(__fdiv_rn(r16(__fmul_rn(conf, rate)), p.max_w));
       const float total = r16(__fadd_rn(tw[i], nw));
       tv[i] = r16(__fdiv_rn(r16(__fadd_rn(r16(__fmul_rn(tv[i], tw[i])), r16(__fmul_rn(nt, nw)))), total));
+      if constexpr (kColor) {
+        // the colour pixel under depth pixel (sx, sy): PyTorch's nearest rule min(floor(s * in / out), in - 1);
+        // c = (c tw + rgb nw) / total with this update's own weights, every op rounded in fp32
+        const int cx = min((int)floorf(__fmul_rn(sx, cp.scale_x)), cp.Wc - 1);
+        const int cy = min((int)floorf(__fmul_rn(sy, cp.scale_y)), cp.Hc - 1);
+        const size_t cpix = (size_t)cp.Hc * cp.Wc;
+        const float* px3 = cp.images + (size_t)b * 3 * cpix + (size_t)cy * cp.Wc + cx;
+#pragma unroll
+        for (int ch = 0; ch < 3; ++ch) {
+          const float rgb = fminf(fmaxf(__fdiv_rn(__fadd_rn(px3[ch * cpix], -cp.mean[ch]), cp.std[ch]), 0.0f), 1.0f);
+          tc[ch][i] = __fdiv_rn(__fadd_rn(__fmul_rn(tc[ch][i], tw[i]), __fmul_rn(rgb, nw)), total);
+        }
+      }
       tw[i] = fminf(total, 1.0f);
       dirty = true;
     }
@@ -193,7 +233,35 @@ tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const 
 #pragma unroll
       for (int j = 0; j < VEC; ++j) { tsdf[base + j] = __float2half_rn(tv[j]); weights[base + j] = __float2half_rn(tw[j]); }
     }
+    if constexpr (kColor) {
+#pragma unroll
+      for (int ch = 0; ch < 3; ++ch) {
+        float* dst = cp.colors + ch * cp.plane + base;
+        if (VEC == 8) {
+          *reinterpret_cast<float4*>(dst) = make_float4(tc[ch][0], tc[ch][1], tc[ch][2], tc[ch][3]);
+          *reinterpret_cast<float4*>(dst + 4) = make_float4(tc[ch][4], tc[ch][5], tc[ch][6], tc[ch][7]);
+        } else {
+#pragma unroll
+          for (int j = 0; j < VEC; ++j) dst[j] = tc[ch][j];
+        }
+      }
+    }
   }
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256)
+tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
+                      const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights) {
+  tsdf_integrate_body<VEC, false>(p, frames, depth, mask, tsdf, weights, TsdfColorParams{});
+}
+
+template <int VEC>
+__global__ void __launch_bounds__(256)
+tsdf_integrate_color_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
+                            const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights,
+                            TsdfColorParams cp) {
+  tsdf_integrate_body<VEC, true>(p, frames, depth, mask, tsdf, weights, cp);
 }
 
 }  // namespace
@@ -201,7 +269,7 @@ tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const 
 size_t tsdf_workspace_bytes(int frames) { return sizeof(TsdfFrame) * (size_t)(frames < kMaxFrames ? frames : kMaxFrames) + 256; }
 
 cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_frames& f, void* workspace,
-                                  cudaStream_t stream) {
+                                  cudaStream_t stream, const srcv_tsdf_color* color) {
   TsdfFrame* frames = reinterpret_cast<TsdfFrame*>(workspace);
   __half* tsdf = reinterpret_cast<__half*>(v.tsdf_values);
   __half* weights = reinterpret_cast<__half*>(v.tsdf_weights);
@@ -223,12 +291,26 @@ cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_fra
     p.max_w = v.max_weight;
     const __half* depth = reinterpret_cast<const __half*>(f.depth) + (size_t)b0 * f.H * f.W;
     const uint8_t* mask = f.depth_mask ? f.depth_mask + (size_t)b0 * f.H * f.W : nullptr;
-    const bool vec = (v.Z % kVec) == 0 && ((reinterpret_cast<uintptr_t>(tsdf) | reinterpret_cast<uintptr_t>(weights)) & 15u) == 0;
+    const uintptr_t cptr = color ? reinterpret_cast<uintptr_t>(color->colors) : 0;
+    const bool vec = (v.Z % kVec) == 0 && ((reinterpret_cast<uintptr_t>(tsdf) | reinterpret_cast<uintptr_t>(weights) | cptr) & 15u) == 0;
     const long long plane = (long long)v.Y * (vec ? v.Z / kVec : v.Z);
     if (plane > 2147483647ll || v.X > 65535) return cudaErrorInvalidValue;
     const dim3 grid((unsigned)((plane + 255) / 256), (unsigned)v.X);
-    if (vec) SRCV_LAUNCH(tsdf_integrate_kernel<kVec>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights);
-    else SRCV_LAUNCH(tsdf_integrate_kernel<1>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights);
+    if (color != nullptr) {
+      TsdfColorParams cp;
+      cp.colors = reinterpret_cast<float*>(color->colors);
+      cp.plane = (size_t)v.X * v.Y * v.Z;
+      cp.Hc = color->Hc; cp.Wc = color->Wc;
+      cp.images = reinterpret_cast<const float*>(color->images) + (size_t)b0 * 3 * color->Hc * color->Wc;
+      cp.scale_x = (float)color->Wc / (float)f.W;
+      cp.scale_y = (float)color->Hc / (float)f.H;
+      for (int ch = 0; ch < 3; ++ch) { cp.mean[ch] = color->mean[ch]; cp.std[ch] = color->std[ch]; }
+      if (vec) SRCV_LAUNCH(tsdf_integrate_color_kernel<kVec>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights, cp);
+      else SRCV_LAUNCH(tsdf_integrate_color_kernel<1>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights, cp);
+    } else {
+      if (vec) SRCV_LAUNCH(tsdf_integrate_kernel<kVec>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights);
+      else SRCV_LAUNCH(tsdf_integrate_kernel<1>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights);
+    }
     note_launch();
     cudaError_t err = cudaGetLastError();
     if (err != cudaSuccess) return err;

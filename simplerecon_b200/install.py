@@ -9,7 +9,10 @@ reference.  ``install(losses=True)`` also swaps the reference's ``losses.MVDepth
 training loss of depth_model.py:144, :477-485) for the kernel-backed mirror.  ``install(fusion=True)``
 swaps ``tools.tsdf.TSDF`` / ``TSDFFuser`` for the kernel-backed mirrors (fusion and mesh export), and
 the names ``tools.fusers_helper`` bound at import (tools/fusers_helper.py:8) if it was already
-imported.  ``uninstall()`` restores everything.  See INTEGRATION.md.
+imported.  ``install(fusion=True, fuse_color=True)`` also wraps ``tools.fusers_helper.get_fuser`` so that
+``--depth_fuser ours --fuse_color`` gets a ``fusers.ColorFuser`` (colour fused on the GPU) instead of the
+reference's warning and a colourless ``OurFuser``; every other option goes to the original.
+``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
 
@@ -20,10 +23,12 @@ _NAMES = ("CostVolumeManager", "FeatureVolumeManager", "FastFeatureVolumeManager
 _saved: dict = {}
 
 
-def install(verbose: bool = False, losses: bool = False, fusion: bool = False) -> list[str]:
+def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
-    with ``fusion=True`` also as ``tools.tsdf``."""
+    with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``."""
+    if fuse_color and not fusion:
+        raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
     from . import cost_volume as ours
     patched = []
     ref_cv = importlib.import_module("modules.cost_volume")
@@ -49,7 +54,7 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False) -
     if fusion:
         from . import tsdf as ours_tsdf
         ref_tsdf = importlib.import_module("tools.tsdf")
-        fh = sys.modules.get("tools.fusers_helper")
+        fh = importlib.import_module("tools.fusers_helper") if fuse_color else sys.modules.get("tools.fusers_helper")
         for mod in [ref_tsdf] + ([fh] if fh is not None else []):
             for n in ("TSDF", "TSDFFuser"):
                 if hasattr(mod, n):
@@ -57,9 +62,28 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False) -
                     setattr(mod, n, getattr(ours_tsdf, n))
             if mod.__name__ not in patched:
                 patched.append(mod.__name__)
+        if fuse_color:
+            _saved.setdefault((fh.__name__, "get_fuser"), fh.get_fuser)
+            fh.get_fuser = _color_get_fuser(_saved[(fh.__name__, "get_fuser")], fh)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched
+
+
+def _color_get_fuser(original, fh):
+    """``get_fuser`` (tools/fusers_helper.py:188-220) with ``ours`` + ``fuse_color`` -> ``ColorFuser``."""
+    def get_fuser(opts, scan):
+        if getattr(opts, "depth_fuser", None) != "ours" or not getattr(opts, "fuse_color", False):
+            return original(opts, scan)
+        from .fusers import ColorFuser
+        if opts.dataset == "scannet":      # the ground-truth mesh path exactly as get_fuser computes it
+            gt_path = fh.ScannetDataset.get_gt_mesh_path(opts.dataset_path, opts.split, scan)
+        else:
+            gt_path = None
+        return ColorFuser(gt_path=gt_path, fusion_resolution=opts.fusion_resolution,
+                          max_fusion_depth=opts.fusion_max_depth, fuse_color=True)
+    get_fuser.__wrapped__ = original
+    return get_fuser
 
 
 def uninstall() -> None:

@@ -258,3 +258,61 @@ def make_mvloss_batch(seed: int = 0, batch: int = 2, views: int = 3, height: int
     return dict(depth_pred_b1hw=torch.stack(pred), cur_depth_b1hw=torch.stack(cur_d), src_depth_bk1hw=torch.stack(src_d),
                 cur_invK_b44=torch.stack(invK), src_K_bk44=torch.stack(srcK), cur_world_T_cam_b44=torch.stack(wTc),
                 src_cam_T_world_bk44=torch.stack(scTw))
+
+
+# one base colour per wall of the ray-cast room: x = 0, x = rx, y = 0, y = ry, z = 0, z = rz
+ROOM_WALL_COLORS = ((0.85, 0.25, 0.20), (0.20, 0.70, 0.30), (0.25, 0.35, 0.90),
+                    (0.90, 0.80, 0.20), (0.70, 0.30, 0.80), (0.20, 0.80, 0.85))
+ROOM_CHECKER_M = 0.5          # checker cell size in world metres
+IMAGENET_MEAN, IMAGENET_STD = (0.485, 0.456, 0.406), (0.229, 0.224, 0.225)
+
+
+def room_wall_color(points: torch.Tensor, room=(4.0, 3.0, 2.6)):
+    """Analytic colour of the room's walls at world points (N,3) (float64): the nearest wall's base colour
+    times a world-space checker (1.0 / 0.6) in the wall's two in-plane coordinates.  Returns (rgb (N,3),
+    wall index (N,), distance to the nearest wall edge (N,), distance to the nearest checker line (N,))."""
+    p = points.double()
+    ext = torch.tensor(room, dtype=torch.float64)
+    d = torch.cat([p, ext - p], 1).abs()                                  # distance to walls 0..5 (x0, y0, z0, x1, ...)
+    wall6 = d.argmin(1)
+    axis = wall6 % 3
+    wall = 2 * axis + wall6 // 3                                          # ROOM_WALL_COLORS order
+    other = torch.stack([torch.tensor([1, 2]), torch.tensor([0, 2]), torch.tensor([0, 1])])[axis]   # (N, 2)
+    q = torch.gather(p, 1, other)                                         # in-plane coordinates
+    qe = torch.gather(ext.expand_as(p), 1, other)
+    edge = torch.minimum(q, qe - q).abs().min(1).values
+    cell = torch.floor(q / ROOM_CHECKER_M)
+    checker = torch.where((cell.sum(1) % 2) == 0, 1.0, 0.6).double()
+    frac = q / ROOM_CHECKER_M - cell
+    line = (torch.minimum(frac, 1 - frac) * ROOM_CHECKER_M).min(1).values
+    rgb = torch.tensor(ROOM_WALL_COLORS, dtype=torch.float64)[wall] * checker[:, None]
+    return rgb, wall, edge, line
+
+
+def make_color_tsdf_case(seed: int = 0, frames: int = 2, voxel_size: float = 0.04, height: int = 192,
+                         width: int = 256, color_hw=(288, 384), room=(4.0, 3.0, 2.6), masked: bool = False) -> dict:
+    """make_tsdf_case (same depth maps, poses and RNG stream) plus colour frames of the same views at
+    ``color_hw``: each pixel's ray through its centre hits a wall whose analytic colour is
+    room_wall_color.  ``color`` is ImageNet-normalised as the dataloader hands images out (B,3,Hc,Wc);
+    ``color_raw`` is the same in [0, 1]."""
+    c = make_tsdf_case(seed=seed, frames=frames, voxel_size=voxel_size, height=height, width=width, room=room,
+                       masked=masked)
+    Hc, Wc = color_hw
+    fx, fy = SCANNET_FX * Wc / 640.0, SCANNET_FY * Hc / 480.0
+    cx, cy = SCANNET_CX * Wc / 640.0, SCANNET_CY * Hc / 480.0
+    v, u = torch.meshgrid(torch.arange(Hc, dtype=torch.float64) + 0.5, torch.arange(Wc, dtype=torch.float64) + 0.5,
+                          indexing="ij")
+    rays = torch.stack([(u - cx) / fx, (v - cy) / fy, torch.ones_like(u)], -1).reshape(-1, 3)
+    ext = torch.tensor(room, dtype=torch.float64)
+    imgs = []
+    for E in c["cam_T_world"].double():
+        Rwc = E[:3, :3].T
+        pos = -(Rwc @ E[:3, 3])
+        d = rays @ Rwc.T
+        t = torch.where(d > 0, (ext - pos) / d.clamp_min(1e-12), -pos / d.clamp_max(-1e-12)).min(-1).values
+        rgb, _, _, _ = room_wall_color(pos + t[:, None] * d, room)
+        imgs.append(rgb.reshape(Hc, Wc, 3).permute(2, 0, 1).float())
+    raw = torch.stack(imgs)
+    mean = torch.tensor(IMAGENET_MEAN).view(1, 3, 1, 1)
+    std = torch.tensor(IMAGENET_STD).view(1, 3, 1, 1)
+    return dict(c, color=((raw - mean) / std).contiguous(), color_raw=raw.contiguous())

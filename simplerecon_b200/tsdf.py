@@ -17,6 +17,11 @@ voxel from the grid index; the property materialises it on demand), a batch of f
 launch (frames are applied in order inside the kernel), ``save`` writes the PLY itself without
 moving the volume to the CPU (the reference's ``save`` calls ``self.cpu()`` first), and there is
 no CPU path: CUDA tensors on an sm_90 device, or an exception.
+
+Colour (DESIGN §4.11, this library's definition: the reference's ``OurFuser`` has none): a volume made
+with ``color=True`` carries an fp32 (3,X,Y,Z) ``tsdf_colors`` volume, ``integrate_depth`` then takes
+``color_b3hw`` and averages it in with the values' own weights (values and weights stay bit-identical to
+the plain path), and ``extract_mesh`` / ``to_mesh`` / ``save`` produce vertex colours.
 """
 from __future__ import annotations
 
@@ -36,15 +41,22 @@ class TSDF:
     VOX_MOD = 8   # final voxel volume dimensions are multiples of 8 (:17)
 
     def __init__(self, tsdf_values: torch.Tensor, tsdf_weights: torch.Tensor, voxel_size: float,
-                 origin: torch.Tensor):
+                 origin: torch.Tensor, colors: torch.Tensor | None = None):
         self.tsdf_values = tsdf_values.half().contiguous()
         self.tsdf_weights = tsdf_weights.half().contiguous()
         self.voxel_size = float(voxel_size)
         self.origin = origin.float()          # kept in fp32: the coordinates are built in fp32 and then halved (:99-110, :92)
+        self.tsdf_colors = None               # (3,X,Y,Z) fp32 R, G, B in [0, 1], or None (DESIGN §4.11)
+        if colors is not None:
+            if tuple(colors.shape) != (3, *self.tsdf_values.shape):
+                raise ValueError(f"colors must be (3, X, Y, Z) = (3, {', '.join(map(str, self.tsdf_values.shape))}), "
+                                 f"got {tuple(colors.shape)}")
+            self.tsdf_colors = colors.float().contiguous()
 
     @classmethod
-    def from_bounds(cls, bounds: dict, voxel_size: float, device="cuda"):
-        """-1 / 0 initialised volume covering ``bounds`` (:70-97)."""
+    def from_bounds(cls, bounds: dict, voxel_size: float, device="cuda", color: bool = False):
+        """-1 / 0 initialised volume covering ``bounds`` (:70-97); ``color=True`` adds a 0-initialised
+        colour volume (12 bytes per voxel)."""
         for key in ("xmin", "xmax", "ymin", "ymax", "zmin", "zmax"):
             if key not in bounds:
                 raise KeyError("Provided bounds dict need to have keys 'xmin', 'xmax', 'ymin', 'ymax', 'zmin', 'zmax'!")
@@ -53,7 +65,8 @@ class TSDF:
         origin = torch.tensor([bounds["xmin"], bounds["ymin"], bounds["zmin"]], dtype=torch.float32)
         values = -torch.ones(dims, dtype=torch.float16, device=device)
         weights = torch.zeros(dims, dtype=torch.float16, device=device)
-        return cls(values, weights, voxel_size, origin)
+        colors = torch.zeros((3, *dims), dtype=torch.float32, device=device) if color else None
+        return cls(values, weights, voxel_size, origin, colors)
 
     @classmethod
     def generate_voxel_coords(cls, origin: torch.Tensor, volume_dims: Tuple[int, int, int], voxel_size: float):
@@ -68,7 +81,7 @@ class TSDF:
                                           self.voxel_size).half()
 
     @classmethod
-    def from_mesh(cls, mesh, voxel_size: float, device="cuda"):
+    def from_mesh(cls, mesh, voxel_size: float, device="cuda", color: bool = False):
         """Volume covering ``mesh.vertices`` plus 3 voxels on every side (:51-67)."""
         verts = np.asarray(mesh.vertices)
         xmax, ymax, zmax = verts.max(0)
@@ -76,14 +89,17 @@ class TSDF:
         bounds = {"xmin": xmin, "xmax": xmax, "ymin": ymin, "ymax": ymax, "zmin": zmin, "zmax": zmax}
         for key, val in bounds.items():
             bounds[key] = val - 3 * voxel_size if "min" in key else val + 3 * voxel_size
-        return cls.from_bounds(bounds, voxel_size, device=device)
+        return cls.from_bounds(bounds, voxel_size, device=device, color=color)
 
     @torch.no_grad()
-    def extract_mesh(self, scale_to_world: bool = True, single_mesh: bool = False):
+    def extract_mesh(self, scale_to_world: bool = True, single_mesh: bool = False, with_colors: bool = False):
         """Marching cubes at level 0 on the GPU (DESIGN §4.10).  Returns ``(verts (V,3) float32,
         faces (F,3) int32, normals (V,3) float32)`` on the volume's device; one host synchronisation
         (the vertex / face counts).  World coordinates use the origin rounded to fp16, as the
-        reference's half ``origin`` does (:34, :154)."""
+        reference's half ``origin`` does (:34, :154).  ``with_colors=True`` (a colour volume only) appends
+        the vertex colours, (V,3) float32 in [0, 1] (DESIGN §4.11); the other three are unchanged."""
+        if with_colors and self.tsdf_colors is None:
+            raise ValueError("with_colors=True needs a colour volume (TSDF.from_bounds(..., color=True))")
         values, weights = self.tsdf_values, self.tsdf_weights
         _require_cuda(values)
         dev = values.device
@@ -106,6 +122,13 @@ class TSDF:
             verts = torch.empty((V, 3), device=dev, dtype=torch.float32)
             normals = torch.empty((V, 3), device=dev, dtype=torch.float32)
             faces = torch.empty((F, 3), device=dev, dtype=torch.int32)
+            if with_colors:
+                colors = torch.empty((V, 3), device=dev, dtype=torch.float32)
+                _native.check(lib.srcv_mesh_extract_color(
+                    C.byref(a), C.c_void_p(self.tsdf_colors.data_ptr()), C.c_void_p(verts.data_ptr() if V else 0),
+                    C.c_void_p(normals.data_ptr() if V else 0), C.c_void_p(colors.data_ptr() if V else 0),
+                    C.c_void_p(faces.data_ptr() if F else 0), V, F, C.c_void_p(ws.data_ptr()), n, stream))
+                return verts, faces, normals, colors
             _native.check(lib.srcv_mesh_extract(C.byref(a), C.c_void_p(verts.data_ptr() if V else 0),
                                                 C.c_void_p(normals.data_ptr() if V else 0),
                                                 C.c_void_p(faces.data_ptr() if F else 0), V, F,
@@ -120,42 +143,82 @@ class TSDF:
         except ImportError as e:
             raise ImportError("TSDF.to_mesh needs trimesh; TSDF.extract_mesh returns the mesh as tensors and "
                               "TSDF.save writes a PLY file without it") from e
+        if self.tsdf_colors is not None:     # vertex colours as uint8 rint(255 c) (DESIGN §4.11)
+            verts, faces, norms, colors = self.extract_mesh(scale_to_world=scale_to_world,
+                                                            single_mesh=export_single_mesh, with_colors=True)
+            return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(),
+                                   normals=norms.cpu().numpy(), vertex_colors=colors_to_u8(colors))
         verts, faces, norms = self.extract_mesh(scale_to_world=scale_to_world, single_mesh=export_single_mesh)
         return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(), normals=norms.cpu().numpy())
 
     def save(self, savepath, filename, save_mesh: bool = True):
         """Writes the mesh to ``savepath/filename`` with ``.bin`` replaced by ``.ply`` (:159-168):
         binary little-endian PLY, float x/y/z vertices, uchar-counted int faces.  Unlike the
-        reference this does not move the volume to the CPU, and it needs no trimesh."""
+        reference this does not move the volume to the CPU, and it needs no trimesh.  A colour volume
+        adds uchar red / green / blue vertex properties."""
         os.makedirs(savepath, exist_ok=True)
         if save_mesh:
-            verts, faces, _ = self.extract_mesh()
-            write_ply(os.path.join(savepath, filename).replace(".bin", ".ply"), verts.cpu().numpy(), faces.cpu().numpy())
+            path = os.path.join(savepath, filename).replace(".bin", ".ply")
+            if self.tsdf_colors is not None:
+                verts, faces, _, colors = self.extract_mesh(with_colors=True)
+                write_ply(path, verts.cpu().numpy(), faces.cpu().numpy(), colors_to_u8(colors))
+            else:
+                verts, faces, _ = self.extract_mesh()
+                write_ply(path, verts.cpu().numpy(), faces.cpu().numpy())
 
     def cuda(self):
         self.tsdf_values = self.tsdf_values.cuda()
         self.tsdf_weights = self.tsdf_weights.cuda()
+        if self.tsdf_colors is not None:
+            self.tsdf_colors = self.tsdf_colors.cuda()
         return self
 
     def cpu(self):
         self.tsdf_values = self.tsdf_values.cpu()
         self.tsdf_weights = self.tsdf_weights.cpu()
+        if self.tsdf_colors is not None:
+            self.tsdf_colors = self.tsdf_colors.cpu()
         return self
 
 
-def write_ply(path, verts: np.ndarray, faces: np.ndarray) -> None:
-    """Binary little-endian PLY: float x, y, z per vertex; a uchar count and int indices per face."""
+def colors_to_u8(colors) -> np.ndarray:
+    """(V,3) colours in [0, 1] -> uint8 rint(255 c) (round half to even), as a host array."""
+    c = colors.detach().cpu().numpy() if torch.is_tensor(colors) else np.asarray(colors)
+    return np.rint(np.float32(255.0) * np.clip(c.astype(np.float32), 0.0, 1.0)).astype(np.uint8)
+
+
+def write_ply(path, verts: np.ndarray, faces: np.ndarray, colors: np.ndarray | None = None) -> None:
+    """Binary little-endian PLY: float x, y, z (and uchar red, green, blue when ``colors`` is given:
+    uint8 as is, floats in [0, 1] through ``colors_to_u8``) per vertex; a uchar count and int indices per
+    face."""
     verts = np.ascontiguousarray(verts, dtype="<f4").reshape(-1, 3)
     faces = np.ascontiguousarray(faces, dtype="<i4").reshape(-1, 3)
+    vprops = "property float x\nproperty float y\nproperty float z\n"
+    if colors is not None:
+        colors = np.asarray(colors)
+        colors = (colors if colors.dtype == np.uint8 else colors_to_u8(colors)).reshape(-1, 3)
+        if len(colors) != len(verts):
+            raise ValueError(f"{len(colors)} colours for {len(verts)} vertices")
+        vprops += "property uchar red\nproperty uchar green\nproperty uchar blue\n"
+        vrec = np.empty(len(verts), dtype=[("p", "<f4", (3,)), ("c", "u1", (3,))])
+        vrec["p"], vrec["c"] = verts, colors
+        vbytes = vrec.tobytes()
+    else:
+        vbytes = verts.tobytes()
     header = ("ply\nformat binary_little_endian 1.0\n"
-              f"element vertex {len(verts)}\nproperty float x\nproperty float y\nproperty float z\n"
+              f"element vertex {len(verts)}\n{vprops}"
               f"element face {len(faces)}\nproperty list uchar int vertex_indices\nend_header\n")
     rec = np.empty(len(faces), dtype=[("n", "u1"), ("v", "<i4", (3,))])
     rec["n"], rec["v"] = 3, faces
     with open(path, "wb") as f:
         f.write(header.encode("ascii"))
-        f.write(verts.tobytes())
+        f.write(vbytes)
         f.write(rec.tobytes())
+
+
+# reverse_imagenet_normalize (reference utils/generic_utils.py:153-159): torchvision's normalize with these
+IMAGENET_REVERSE_MEAN = (-2.11790393, -2.03571429, -1.80444444)
+IMAGENET_REVERSE_STD = (4.36681223, 4.46428571, 4.44444444)
 
 
 def _require_cuda(t: torch.Tensor) -> None:
@@ -180,16 +243,28 @@ class TSDFFuser:
     voxel_coords = property(lambda self: self.tsdf.voxel_coords)
     tsdf_values = property(lambda self: self.tsdf.tsdf_values)
     tsdf_weights = property(lambda self: self.tsdf.tsdf_weights)
+    tsdf_colors = property(lambda self: self.tsdf.tsdf_colors)
     voxel_size = property(lambda self: self.tsdf.voxel_size)
     shape = property(lambda self: self.tsdf.tsdf_values.shape)
     truncation = property(lambda self: self.truncation_size * self.voxel_size)
 
     @torch.no_grad()
     def integrate_depth(self, depth_b1hw: torch.Tensor, cam_T_world_T_b44: torch.Tensor, K_b44: torch.Tensor,
-                        depth_mask_b1hw: torch.Tensor | None = None) -> None:
+                        depth_mask_b1hw: torch.Tensor | None = None, color_b3hw: torch.Tensor | None = None,
+                        color_normalized: bool = True) -> None:
         """In-place update of the volume with a batch of depth maps, applied in order (:221-320).
-        Inputs are taken to fp16 as ``OurFuser.fuse_frames`` does (fusers_helper.py:64-71)."""
+        Inputs are taken to fp16 as ``OurFuser.fuse_frames`` does (fusers_helper.py:64-71).
+
+        ``color_b3hw`` (required on a colour volume, refused on a plain one): (B,3,Hc,Wc) images of any
+        size, taken to fp32; ``color_normalized=True`` means ImageNet-normalised as the dataloader hands
+        them out (undone with ``reverse_imagenet_normalize``'s constants), False means already in [0, 1].
+        The kernel picks each update's colour pixel with PyTorch's ``nearest`` rule (DESIGN §4.11)."""
         values, weights = self.tsdf.tsdf_values, self.tsdf.tsdf_weights
+        colors = self.tsdf.tsdf_colors
+        if colors is None and color_b3hw is not None:
+            raise ValueError("color_b3hw given for a volume without colour (TSDF.from_bounds(..., color=True))")
+        if colors is not None and color_b3hw is None:
+            raise ValueError("this volume fuses colour: integrate_depth needs color_b3hw")
         _require_cuda(values)
         dev = values.device
         lib = _native.load()
@@ -209,9 +284,21 @@ class TSDFFuser:
         fr = _native.TsdfFrames(depth.data_ptr(), E.data_ptr(), K.data_ptr(),
                                 mask.data_ptr() if mask is not None else None, B, H, W,
                                 float(self.min_depth), float(self.max_depth))
+        col = None
+        if colors is not None:
+            if color_b3hw.dim() != 4 or color_b3hw.shape[0] != B or color_b3hw.shape[1] != 3:
+                raise ValueError(f"color_b3hw must be ({B}, 3, Hc, Wc), got {tuple(color_b3hw.shape)}")
+            image = color_b3hw.to(dev).float().contiguous()
+            mean, std = (IMAGENET_REVERSE_MEAN, IMAGENET_REVERSE_STD) if color_normalized else ((0.0,) * 3, (1.0,) * 3)
+            col = _native.TsdfColor(colors.data_ptr(), image.data_ptr(), int(image.shape[2]), int(image.shape[3]),
+                                    (C.c_float * 3)(*mean), (C.c_float * 3)(*std))
         with torch.cuda.device(dev):
             n = lib.srcv_tsdf_workspace_bytes(C.byref(fr))
             ws = torch.empty(n, device=dev, dtype=torch.uint8)
-            _native.check(lib.srcv_tsdf_integrate_f16(
-                C.byref(vol), C.byref(fr), C.c_void_p(ws.data_ptr()), n,
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+            stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+            if col is not None:
+                _native.check(lib.srcv_tsdf_integrate_color_f16(C.byref(vol), C.byref(fr), C.byref(col),
+                                                                C.c_void_p(ws.data_ptr()), n, stream))
+            else:
+                _native.check(lib.srcv_tsdf_integrate_f16(C.byref(vol), C.byref(fr), C.c_void_p(ws.data_ptr()), n,
+                                                          stream))
