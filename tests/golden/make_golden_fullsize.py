@@ -1,4 +1,5 @@
-"""Golden vectors at the BENCH feature-map size (120 x 160, 7 views) from the UNMODIFIED reference.
+"""Golden vectors at the BENCH feature-map size (120 x 160, 7 views) and at the reference's default
+matching-feature size (96 x 128, 512 x 384 frames) from the UNMODIFIED reference.
 
     python tests/golden/make_golden_fullsize.py          (needs $SIMPLERECON_REF)
 
@@ -66,3 +67,9 @@ if __name__ == "__main__":
     gen = dict(batch=1, views=7, height=120, width=160, channels=16, seed=4321)
     run_case(R, "full_dot_120x160_D4_K7", "dot", gen, 4)
     run_case(R, "full_hero_120x160_D4_K7", "mlp", dict(gen, seed=4322), 4)
+    # 512 x 384 frames, the reference's default resolution: the kernels' compile-time 128 x 96
+    # instantiations.  D = 5 for the MLP puts the last plane (the one that carries the mask) in a
+    # partial two-plane tile.
+    gen96 = dict(gen, height=96, width=128)
+    run_case(R, "full_dot_96x128_D4_K7", "dot", dict(gen96, seed=4323), 4)
+    run_case(R, "full_hero_96x128_D5_K7", "mlp", dict(gen96, seed=4324), 5)
