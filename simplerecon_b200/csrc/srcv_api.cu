@@ -97,6 +97,20 @@ static int32_t check_workspace(void* ws, size_t have, size_t need) {
   return SRCV_OK;
 }
 
+// Checks the caller's workspace against what this call needs, then carves it.
+static int32_t take_workspace(const srcv_shape& s, void* base, size_t have, bool want_c4, size_t extra,
+                              Workspace& ws) {
+  if (int32_t e = check_workspace(base, have, carve_workspace(s, nullptr, want_c4, extra).bytes)) return e;
+  ws = carve_workspace(s, base, want_c4, extra);
+  return SRCV_OK;
+}
+
+// The plane depths a sweep reads: the prep kernel's (B,D) copy for FROM_RANGE, else the caller's.
+struct SweepPlanes { const float* planes; bool per_pixel; };
+static SweepPlanes sweep_planes(const srcv_planes& pl, const Workspace& ws) {
+  return {pl.mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl.planes, pl.mode == SRCV_PLANES_PER_PIXEL};
+}
+
 static bool use_fast_dot(const srcv_shape& s) {
   const int v = g_variant.load();
   if (v == SRCV_VARIANT_GENERIC) return false;
@@ -162,9 +176,8 @@ int32_t srcv_dot_forward_f32(const srcv_shape* s, const float* cur, const float*
     return fail(SRCV_ERR_UNSUPPORTED, "fast dot variant needs C == 16 and K <= 8");
   if (s->layout == SRCV_LAYOUT_CHUNK_PLANAR && !fast)
     return fail(SRCV_ERR_UNSUPPORTED, "chunk-planar features are served by the chunk-planar dot sweep only (C == 16, variant != generic)");
-  const Workspace need = carve_workspace(*s, nullptr, dot_fast_supported(*s), 0);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, need.bytes)) return e;
-  Workspace ws = carve_workspace(*s, workspace, dot_fast_supported(*s), 0);
+  Workspace ws;
+  if (int32_t e = take_workspace(*s, workspace, workspace_bytes, dot_fast_supported(*s), 0, ws)) return e;
   if (!fast) { ws.src_c4 = nullptr; ws.tile_done = nullptr; }  // skip the chunk-planar copies
   ws.cur_c4 = nullptr;             // the dot kernel keeps the reference features in registers
   if (s->layout == SRCV_LAYOUT_CHUNK_PLANAR) ws.src_c4 = const_cast<float*>(src);   // gathered in place, no copy
@@ -174,14 +187,13 @@ int32_t srcv_dot_forward_f32(const srcv_shape* s, const float* cur, const float*
   cudaError_t err = launch_prep(*s, *cams, *pl, src, cur, ws, false, stream);
   if (err != cudaSuccess) return cuda_fail(err, "prep");
   if (pr) cudaEventRecord(pr->e[1], stream);
-  const bool per_pixel = pl->mode == SRCV_PLANES_PER_PIXEL;
-  const float* planes = pl->mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl->planes;
+  const SweepPlanes sp = sweep_planes(*pl, ws);
   if (fast) {
     g_last_variant.store("dot_fast_c4planar");
-    err = launch_dot_fast(*s, cur, ws, planes, per_pixel, cost, lowest, stream);
+    err = launch_dot_fast(*s, cur, ws, sp.planes, sp.per_pixel, cost, lowest, stream);
   } else {
     g_last_variant.store("dot_generic");
-    err = launch_dot_generic(*s, cur, src, ws, planes, per_pixel, cost, lowest, stream);
+    err = launch_dot_generic(*s, cur, src, ws, sp.planes, sp.per_pixel, cost, lowest, stream);
   }
   if (err != cudaSuccess) return cuda_fail(err, g_last_variant.load());
   if (pr) cudaEventRecord(pr->e[2], stream);
@@ -206,18 +218,16 @@ int32_t srcv_dot_backward_f32(const srcv_shape* s, const float* cur, const float
   if (!dot_backward_supported(*s))
     return fail(SRCV_ERR_UNSUPPORTED, "dot backward is built for C in {8, 16, 32}, got %d", s->C);
   if (s->layout != SRCV_LAYOUT_NCHW) return fail(SRCV_ERR_UNSUPPORTED, "the backward kernels take NCHW features");
-  const Workspace need = carve_workspace(*s, nullptr, false, 0);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, need.bytes)) return e;
-  Workspace ws = carve_workspace(*s, workspace, false, 0);
+  Workspace ws;
+  if (int32_t e = take_workspace(*s, workspace, workspace_bytes, false, 0, ws)) return e;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   cudaError_t err = launch_prep(*s, *cams, *pl, src, cur, ws, false, stream);
   if (err != cudaSuccess) return cuda_fail(err, "prep");
   err = cudaMemsetAsync(grad_src, 0, sizeof(float) * (size_t)s->B * s->K * s->C * s->H * s->W, stream);
   if (err != cudaSuccess) return cuda_fail(err, "memset grad_src");
-  const bool per_pixel = pl->mode == SRCV_PLANES_PER_PIXEL;
-  const float* planes = pl->mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl->planes;
+  const SweepPlanes sp = sweep_planes(*pl, ws);
   g_last_variant.store("dot_backward_atomic");
-  err = launch_dot_backward(*s, cur, src, ws, planes, per_pixel, grad_cost, grad_cur, grad_src, stream);
+  err = launch_dot_backward(*s, cur, src, ws, sp.planes, sp.per_pixel, grad_cost, grad_cur, grad_src, stream);
   if (err != cudaSuccess) return cuda_fail(err, g_last_variant.load());
   return SRCV_OK;
 }
@@ -238,9 +248,8 @@ static int32_t warp_planes_impl(const srcv_shape* s, const float* src, const src
     return fail(SRCV_ERR_NULL, "camera block incomplete");
   if (s->layout != SRCV_LAYOUT_NCHW) return fail(SRCV_ERR_UNSUPPORTED, "warp_features takes NCHW features");
   if (s->D > 65535) return fail(SRCV_ERR_SHAPE, "at most 65535 planes per warp call");
-  const Workspace need = carve_workspace(*s, nullptr, false, 0);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, need.bytes)) return e;
-  Workspace ws = carve_workspace(*s, workspace, false, 0);
+  Workspace ws;
+  if (int32_t e = take_workspace(*s, workspace, workspace_bytes, false, 0, ws)) return e;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   srcv_planes pl{};
   pl.mode = SRCV_PLANES_PER_PLANE;   // the planes come straight from the caller
@@ -331,9 +340,8 @@ int32_t srcv_mlp_forward_f32(const srcv_shape* s, const float* cur, const float*
     return fail(SRCV_ERR_UNSUPPORTED, "chunk-planar features are served by the tensor-core MLP sweep only (K == 7, C == 16, 128/128, variant != generic)");
   const size_t extra = mlp_extra_bytes(*s, *w);
   const bool c4 = mlp_tc_supported(*s, *w);
-  const Workspace need = carve_workspace(*s, nullptr, c4, extra);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, need.bytes)) return e;
-  Workspace ws = carve_workspace(*s, workspace, c4, extra);
+  Workspace ws;
+  if (int32_t e = take_workspace(*s, workspace, workspace_bytes, c4, extra, ws)) return e;
   if (!tc) ws.src_c4 = nullptr;  // skip the chunk-planar copy
   ws.tile_done = nullptr;        // only the dot sweep uses the tile counters
   if (s->layout == SRCV_LAYOUT_CHUNK_PLANAR) {   // gathered in place, no copy
@@ -346,14 +354,13 @@ int32_t srcv_mlp_forward_f32(const srcv_shape* s, const float* cur, const float*
   cudaError_t err = launch_prep(*s, *cams, *pl, src, cur, ws, true, stream);
   if (err != cudaSuccess) return cuda_fail(err, "prep");
   if (pr) cudaEventRecord(pr->e[1], stream);
-  const bool per_pixel = pl->mode == SRCV_PLANES_PER_PIXEL;
-  const float* planes = pl->mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl->planes;
+  const SweepPlanes sp = sweep_planes(*pl, ws);
   if (tc) {
     g_last_variant.store("mlp_tc_wgmma_f16x3");
-    err = launch_mlp_tc(*s, cur, ws, planes, per_pixel, *w, cost, lowest, overall_mask, stream);
+    err = launch_mlp_tc(*s, cur, ws, sp.planes, sp.per_pixel, *w, cost, lowest, overall_mask, stream);
   } else {
     g_last_variant.store("mlp_generic_fp32");
-    err = launch_mlp_generic(*s, cur, src, ws, planes, per_pixel, *w, cost, lowest, overall_mask, stream);
+    err = launch_mlp_generic(*s, cur, src, ws, sp.planes, sp.per_pixel, *w, cost, lowest, overall_mask, stream);
   }
   if (err != cudaSuccess) return cuda_fail(err, g_last_variant.load());
   if (pr) cudaEventRecord(pr->e[2], stream);
@@ -387,14 +394,13 @@ int32_t srcv_mlp_backward_f32(const srcv_shape* s, const float* cur, const float
   if (!mlp_backward_supported(*s, *w))
     return fail(SRCV_ERR_UNSUPPORTED, "MLP backward supports at most 208 input features and hidden widths <= 128");
   if (s->layout != SRCV_LAYOUT_NCHW) return fail(SRCV_ERR_UNSUPPORTED, "the backward kernels take NCHW features");
-  const size_t extra = mlp_backward_extra_bytes(*s, *w);
-  const Workspace need = carve_workspace(*s, nullptr, false, extra);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, need.bytes)) return e;
-  Workspace ws = carve_workspace(*s, workspace, false, extra);
+  Workspace ws;
+  if (int32_t e = take_workspace(*s, workspace, workspace_bytes, false, mlp_backward_extra_bytes(*s, *w), ws))
+    return e;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   cudaError_t err = launch_prep(*s, *cams, *pl, src, cur, ws, true, stream);
   if (err != cudaSuccess) return cuda_fail(err, "prep");
-  const size_t F = (size_t)s->C * (s->K + 1) + 10 * (size_t)s->K + 4;
+  const size_t F = mlp_features(s->K, s->C);
   const size_t HW = (size_t)s->H * s->W;
   struct { void* p; size_t n; } zero[] = {
       {grad_cur, (size_t)s->B * s->C * HW}, {grad_src, (size_t)s->B * s->K * s->C * HW},
@@ -405,10 +411,9 @@ int32_t srcv_mlp_backward_f32(const srcv_shape* s, const float* cur, const float
     err = cudaMemsetAsync(z.p, 0, sizeof(float) * z.n, stream);
     if (err != cudaSuccess) return cuda_fail(err, "memset gradients");
   }
-  const bool per_pixel = pl->mode == SRCV_PLANES_PER_PIXEL;
-  const float* planes = pl->mode == SRCV_PLANES_FROM_RANGE ? ws.planes : pl->planes;
+  const SweepPlanes sp = sweep_planes(*pl, ws);
   g_last_variant.store("mlp_backward_fp32_recompute");
-  err = launch_mlp_backward(*s, cur, src, ws, planes, per_pixel, *w, grad_cost, grad_cur, grad_src, *g, stream);
+  err = launch_mlp_backward(*s, cur, src, ws, sp.planes, sp.per_pixel, *w, grad_cost, grad_cur, grad_src, *g, stream);
   if (err != cudaSuccess) return cuda_fail(err, g_last_variant.load());
   return SRCV_OK;
 }

@@ -29,6 +29,8 @@
 #endif
 #include <stdint.h>
 
+#include "../../include/srcv_b200.h"
+
 // Dynamic shared memory of a kernel (one definition so the host emulation can map it).
 #ifdef SRCV_HOST_EMU
 #define SRCV_DYNAMIC_SMEM(type, name) type* name = reinterpret_cast<type*>(::emu::dynamic_smem())
@@ -166,6 +168,115 @@ __device__ __forceinline__ void argmax_update(float v, float dval, float& best, 
                                               bool first) {
   const bool take = first || (v > best) || ((v != v) && (best == best));
   if (take) { best = v; best_d = dval; }
+}
+
+// Depth of plane d of frame b at pixel p: per-pixel (B,D,H,W) or per-plane (B,D) planes.
+template <bool PER_PIXEL>
+__device__ __forceinline__ float plane_depth(const float* __restrict__ planes, int b, int D, int d, int HW, int p) {
+  return PER_PIXEL ? __ldg(planes + ((size_t)b * D + d) * HW + p) : __ldg(planes + b * D + d);
+}
+
+// One projected (pixel, view) sample: footprint, bilinear weights, z' and the depth mask.
+struct Sample {
+  Taps tp;
+  float w00, w01, w10, w11;
+  float px, py, zp, mk;
+};
+
+// `vp` is a view's a0 | hx | hy | t (ViewParams, or its kViewFloats shared-memory copy);
+// dx, dy is the pixel centre relative to the image centre.
+__device__ __forceinline__ Sample project_sample(const float* __restrict__ vp, const Centre& ctr, int W, int H,
+                                                 float dx, float dy, float dval) {
+  Sample sm;
+  float ax, ay, az;
+  homography_point(vp, dx, dy, ax, ay, az);
+  project_point(dval, ax, ay, az, vp[9], vp[10], vp[11], sm.px, sm.py, sm.zp);
+  bilinear_taps(sm.px, sm.py, W, H, ctr, sm.tp);
+  sm.w00 = (1.0f - sm.tp.fx) * (1.0f - sm.tp.fy);
+  sm.w01 = sm.tp.fx * (1.0f - sm.tp.fy);
+  sm.w10 = (1.0f - sm.tp.fx) * sm.tp.fy;
+  sm.w11 = sm.tp.fx * sm.tp.fy;
+  sm.mk = sm.zp > 0.0f ? 1.0f : 0.0f;
+  return sm;
+}
+
+// Bilinear blend of one channel plane at the sample's footprint (zeros padding).
+__device__ __forceinline__ float gather4(const float* __restrict__ q, int W, const Sample& sm) {
+  float v = 0.f;
+  if (sm.tp.valid & 1u) v = sm.w00 * __ldg(q);
+  if (sm.tp.valid & 2u) v = fmaf(sm.w01, __ldg(q + 1), v);
+  if (sm.tp.valid & 4u) v = fmaf(sm.w10, __ldg(q + W), v);
+  if (sm.tp.valid & 8u) v = fmaf(sm.w11, __ldg(q + W + 1), v);
+  return v;
+}
+
+// ---- the metadata row: the MLP input of modules/cost_volume.py:590-723 ------------------------
+// Channels of K views with C features each: C (K+1) + 10 K + 4.
+constexpr __host__ __device__ int mlp_features(int K, int C) { return C * (K + 1) + 10 * K + 4; }
+
+// Channel offsets: K*C warped features, then cur (C), mask (K), z' (K), depth (1), masked dot (K),
+// ray angle (K), n_cur (3), n_src (3K), pose distance, rotation and translation measures (K each).
+struct MetaLayout {
+  int cur, mask, z, depth, dot, ang, ncur, nsrc, comb, r, t;
+  __device__ MetaLayout(int K, int C)
+      : cur(K * C), mask(cur + C), z(mask + K), depth(z + K), dot(depth + 1), ang(dot + K), ncur(ang + K),
+        nsrc(ncur + 3), comb(nsrc + 3 * K), r(comb + K), t(r + K) {}
+};
+
+// Writes view k's channels of pixel p's row into the feature-major shared tile[channel * pitch + row].
+// View 0 also writes the view-independent channels (reference features, depth, n_cur) and zeroes the
+// padding channels [F, f_end).  Features are sampled even behind the camera; only the dot is masked.
+// Returns the view's sample (the forward takes its mask bits from it).
+__device__ __forceinline__ Sample metadata_row(float* __restrict__ tile, int pitch, int row, int F, int f_end,
+                                               const MetaLayout& o, const srcv_shape& s,
+                                               const float* __restrict__ cur, const float* __restrict__ src,
+                                               const ViewParams& vp, const FrameParams& fp, int b, int k, int p,
+                                               float dval) {
+  const int HW = s.H * s.W, K = s.K, C = s.C;
+  const Centre ctr(s.W, s.H);
+  const float pxc = (float)(p % s.W) + 0.5f, pyc = (float)(p / s.W) + 0.5f;
+  const Sample sm = project_sample(vp.a0, ctr, s.W, s.H, pxc - ctr.half_w, pyc - ctr.half_h, dval);
+  // warped features + per-view dot
+  const float* sp = src + ((size_t)(b * K + k) * C) * HW + (sm.tp.y0 * s.W + sm.tp.x0);
+  const float* cp = cur + (size_t)b * C * HW + p;
+  float dot = 0.f;
+  for (int c = 0; c < C; ++c) {
+    const float v = gather4(sp + (size_t)c * HW, s.W, sm);
+    tile[(k * C + c) * pitch + row] = v;
+    dot = fmaf(v, __ldg(cp + (size_t)c * HW), dot);
+  }
+  tile[(o.mask + k) * pitch + row] = sm.mk;
+  tile[(o.z + k) * pitch + row] = sm.zp;
+  tile[(o.dot + k) * pitch + row] = dot * sm.mk;
+  // rays: X = d * (invK3 p); n_cur = X/|X|; n_src = (X - centre_k)/|.|
+  const float rx = fmaf(fp.invK[0], pxc, fmaf(fp.invK[1], pyc, fp.invK[2]));
+  const float ry = fmaf(fp.invK[3], pxc, fmaf(fp.invK[4], pyc, fp.invK[5]));
+  const float rz = fmaf(fp.invK[6], pxc, fmaf(fp.invK[7], pyc, fp.invK[8]));
+  const float X = dval * rx, Y = dval * ry, Z = dval * rz;
+  const float nc = fmaxf(sqrtf(fmaf(X, X, fmaf(Y, Y, Z * Z))), kEpsNorm);
+  const float cx = X / nc, cy = Y / nc, cz = Z / nc;
+  const float sx0 = X - vp.centre[0], sy0 = Y - vp.centre[1], sz0 = Z - vp.centre[2];
+  const float ns = fmaxf(sqrtf(fmaf(sx0, sx0, fmaf(sy0, sy0, sz0 * sz0))), kEpsNorm);
+  const float sx = sx0 / ns, sy = sy0 / ns, sz = sz0 / ns;
+  // cosine_similarity(eps=1e-5) of the two (already unit) rays
+  const float n1 = fmaxf(sqrtf(fmaf(cx, cx, fmaf(cy, cy, cz * cz))), kEpsCos);
+  const float n2 = fmaxf(sqrtf(fmaf(sx, sx, fmaf(sy, sy, sz * sz))), kEpsCos);
+  tile[(o.ang + k) * pitch + row] = fmaf(cx / n1, sx / n2, fmaf(cy / n1, sy / n2, (cz / n1) * (sz / n2)));
+  tile[(o.nsrc + 3 * k + 0) * pitch + row] = sx;
+  tile[(o.nsrc + 3 * k + 1) * pitch + row] = sy;
+  tile[(o.nsrc + 3 * k + 2) * pitch + row] = sz;
+  tile[(o.comb + k) * pitch + row] = vp.comb;
+  tile[(o.r + k) * pitch + row] = vp.rmeas;
+  tile[(o.t + k) * pitch + row] = vp.tmeas;
+  if (k == 0) {
+    for (int c = 0; c < C; ++c) tile[(o.cur + c) * pitch + row] = __ldg(cp + (size_t)c * HW);
+    tile[o.depth * pitch + row] = dval;
+    tile[(o.ncur + 0) * pitch + row] = cx;
+    tile[(o.ncur + 1) * pitch + row] = cy;
+    tile[(o.ncur + 2) * pitch + row] = cz;
+    for (int f = F; f < f_end; ++f) tile[f * pitch + row] = 0.f;
+  }
+  return sm;
 }
 
 }  // namespace srcv

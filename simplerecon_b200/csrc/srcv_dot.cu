@@ -48,30 +48,14 @@ dot_generic_kernel(srcv_shape s, const float* __restrict__ cur, const float* __r
   const float* curp = cur + (size_t)b * s.C * HW + p;
   float best = 0.f, best_d = 0.f;
   for (int d = 0; d < s.D; ++d) {
-    const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p)
-                                 : __ldg(planes + b * s.D + d);
+    const float dval = plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p);
     float acc = 0.f;
     for (int k = 0; k < s.K; ++k) {
-      const float* vp = sview + k * kViewFloats;
-      float ax, ay, az, px, py, zp;
-      homography_point(vp, dx, dy, ax, ay, az);
-      project_point(dval, ax, ay, az, vp[9], vp[10], vp[11], px, py, zp);
-      Taps tp;
-      bilinear_taps(px, py, s.W, s.H, ctr, tp);
-      if (!(zp > 0.0f) || tp.valid == 0u) continue;  // mask == 0 or all taps padded
-      const float w00 = (1.0f - tp.fx) * (1.0f - tp.fy), w01 = tp.fx * (1.0f - tp.fy);
-      const float w10 = (1.0f - tp.fx) * tp.fy, w11 = tp.fx * tp.fy;
-      const float* sp = src + ((size_t)(b * s.K + k) * s.C) * HW + (tp.y0 * s.W + tp.x0);
+      const Sample sm = project_sample(sview + k * kViewFloats, ctr, s.W, s.H, dx, dy, dval);
+      if (!(sm.zp > 0.0f) || sm.tp.valid == 0u) continue;  // mask == 0 or all taps padded
+      const float* sp = src + ((size_t)(b * s.K + k) * s.C) * HW + (sm.tp.y0 * s.W + sm.tp.x0);
       float dot = 0.f;
-      for (int c = 0; c < s.C; ++c) {
-        const float* q = sp + (size_t)c * HW;
-        float v = 0.f;
-        if (tp.valid & 1u) v = w00 * __ldg(q);
-        if (tp.valid & 2u) v = fmaf(w01, __ldg(q + 1), v);
-        if (tp.valid & 4u) v = fmaf(w10, __ldg(q + s.W), v);
-        if (tp.valid & 8u) v = fmaf(w11, __ldg(q + s.W + 1), v);
-        dot = fmaf(v, __ldg(curp + (size_t)c * HW), dot);
-      }
+      for (int c = 0; c < s.C; ++c) dot = fmaf(gather4(sp + (size_t)c * HW, s.W, sm), __ldg(curp + (size_t)c * HW), dot);
       acc += dot;
     }
     cost[((size_t)b * s.D + d) * HW + p] = acc;
@@ -271,32 +255,17 @@ warp_planes_kernel(srcv_shape s, const float* __restrict__ src, const ViewParams
   if (p >= HW) return;
   const Centre ctr(s.W, s.H);
   const float dx = ((float)(p % s.W) + 0.5f) - ctr.half_w, dy = ((float)(p / s.W) + 0.5f) - ctr.half_h;
-  const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p) : __ldg(planes + b * s.D + d);
-  const ViewParams& vp = views[bk];
-  float ax, ay, az, px, py, zp;
-  homography_point(vp.a0, dx, dy, ax, ay, az);
-  project_point(dval, ax, ay, az, vp.t[0], vp.t[1], vp.t[2], px, py, zp);
-  Taps tp;
-  bilinear_taps(px, py, s.W, s.H, ctr, tp);
-  const float w00 = (1.0f - tp.fx) * (1.0f - tp.fy), w01 = tp.fx * (1.0f - tp.fy);
-  const float w10 = (1.0f - tp.fx) * tp.fy, w11 = tp.fx * tp.fy;
-  const float* sp = src + (size_t)bk * s.C * HW + (tp.y0 * s.W + tp.x0);
+  const float dval = plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p);
+  const Sample sm = project_sample(views[bk].a0, ctr, s.W, s.H, dx, dy, dval);
+  const float* sp = src + (size_t)bk * s.C * HW + (sm.tp.y0 * s.W + sm.tp.x0);
   const size_t o = (size_t)bk * s.D + d;
-  for (int c = 0; c < s.C; ++c) {
-    const float* q = sp + (size_t)c * HW;
-    float v = 0.f;
-    if (tp.valid & 1u) v = w00 * __ldg(q);
-    if (tp.valid & 2u) v = fmaf(w01, __ldg(q + 1), v);
-    if (tp.valid & 4u) v = fmaf(w10, __ldg(q + s.W), v);
-    if (tp.valid & 8u) v = fmaf(w11, __ldg(q + s.W + 1), v);
-    warped[(o * s.C + c) * HW + p] = v;
-  }
-  depths[o * HW + p] = zp;
-  mask[o * HW + p] = zp > 0.0f ? 1.0f : 0.0f;
+  for (int c = 0; c < s.C; ++c) warped[(o * s.C + c) * HW + p] = gather4(sp + (size_t)c * HW, s.W, sm);
+  depths[o * HW + p] = sm.zp;
+  mask[o * HW + p] = sm.mk;
   if (pix != nullptr) {
     // the projector's pixel coordinates (utils/geometry_utils.py:88-89): ours are centred
-    pix[(o * 2 + 0) * HW + p] = px + ((float)ctr.nx + 0.5f);
-    pix[(o * 2 + 1) * HW + p] = py + ((float)ctr.ny + 0.5f);
+    pix[(o * 2 + 0) * HW + p] = sm.px + ((float)ctr.nx + 0.5f);
+    pix[(o * 2 + 1) * HW + p] = sm.py + ((float)ctr.ny + 0.5f);
   }
 }
 

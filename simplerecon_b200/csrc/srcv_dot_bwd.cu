@@ -45,16 +45,12 @@ dot_backward_kernel(srcv_shape s, const float* __restrict__ cur, const float* __
   for (int d = d_begin; d < d_end; ++d) {
     const float g = __ldg(gcost + ((size_t)b * s.D + d) * HW + p);
     if (g == 0.0f) continue;
-    const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p)
-                                 : __ldg(planes + b * s.D + d);
+    const float dval = plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p);
     for (int k = 0; k < K; ++k) {
-      const float* vp = sview + k * kViewFloats;
-      float ax, ay, az, px, py, zp;
-      homography_point(vp, dx, dy, ax, ay, az);
-      project_point(dval, ax, ay, az, vp[9], vp[10], vp[11], px, py, zp);
-      Taps tp;
-      bilinear_taps(px, py, W, H, ctr, tp);
-      if (!(zp > 0.0f) || tp.valid == 0u) continue;
+      const Sample sm = project_sample(sview + k * kViewFloats, ctr, W, H, dx, dy, dval);
+      const Taps& tp = sm.tp;
+      if (!(sm.zp > 0.0f) || tp.valid == 0u) continue;
+      // own weights: g * gx * gy rounds differently from g * sm.w00 = g * (gx * gy)
       const float gx = 1.0f - tp.fx, gy = 1.0f - tp.fy;
       const float wgt[4] = {g * gx * gy, g * tp.fx * gy, g * gx * tp.fy, g * tp.fx * tp.fy};
       const int off[4] = {0, 1, W, W + 1};

@@ -12,8 +12,8 @@
 //
 // Nothing of the forward is saved: a persistent CTA walks 64-row tiles (64 consecutive
 // pixels of one frame at one depth plane) and for each tile
-//   1. rebuilds the 64 x F metadata tile X in shared memory (same arithmetic as the
-//      forward kernels, srcv_common.cuh),
+//   1. rebuilds the 64 x F metadata tile X in shared memory (metadata_row of
+//      srcv_common.cuh, the builder of the SIMT forward),
 //   2. re-runs  A1 = X W1^T + b1, H1 = lrelu(A1),  A2 = H1 W2^T + b2  (register-tiled fp32),
 //   3. forms  G2 = g (x) w3 . lrelu'(A2)  in registers,  dW3 += g^T H2,  db3 += sum g,
 //      db2 += sum_r G2,  dW2 += G2^T H1,
@@ -168,35 +168,6 @@ __device__ __forceinline__ void grad_outer(const float* __restrict__ sA, const f
   }
 }
 
-// Projection of one (row, view) sample: footprint, bilinear weights, z' and the depth mask.
-struct Sample {
-  Taps tp;
-  float w00, w01, w10, w11;
-  float px, py, zp, mk;
-};
-
-__device__ __forceinline__ void project_sample(const ViewParams& vp, const Centre& ctr, int W, int H,
-                                               float pxc, float pyc, float dval, Sample& sm) {
-  float ax, ay, az;
-  homography_point(vp.a0, pxc - ctr.half_w, pyc - ctr.half_h, ax, ay, az);
-  project_point(dval, ax, ay, az, vp.t[0], vp.t[1], vp.t[2], sm.px, sm.py, sm.zp);
-  bilinear_taps(sm.px, sm.py, W, H, ctr, sm.tp);
-  sm.w00 = (1.0f - sm.tp.fx) * (1.0f - sm.tp.fy);
-  sm.w01 = sm.tp.fx * (1.0f - sm.tp.fy);
-  sm.w10 = (1.0f - sm.tp.fx) * sm.tp.fy;
-  sm.w11 = sm.tp.fx * sm.tp.fy;
-  sm.mk = sm.zp > 0.0f ? 1.0f : 0.0f;
-}
-
-__device__ __forceinline__ float gather4(const float* __restrict__ q, int W, const Sample& sm) {
-  float v = 0.f;
-  if (sm.tp.valid & 1u) v = sm.w00 * __ldg(q);
-  if (sm.tp.valid & 2u) v = fmaf(sm.w01, __ldg(q + 1), v);
-  if (sm.tp.valid & 4u) v = fmaf(sm.w10, __ldg(q + W), v);
-  if (sm.tp.valid & 8u) v = fmaf(sm.w11, __ldg(q + W + 1), v);
-  return v;
-}
-
 template <bool PER_PIXEL, int NIF>
 __global__ void __launch_bounds__(BNT, 1)
 mlp_backward_kernel(srcv_shape s, BwdDims m, const float* __restrict__ cur,
@@ -219,9 +190,7 @@ mlp_backward_kernel(srcv_shape s, BwdDims m, const float* __restrict__ cur,
   float* sRed = sGo + BT;         // [BN + 1] dW3 partials, db3
   const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
   const int HW = s.H * s.W, K = s.K, C = s.C;
-  const int o_cur = K * C, o_mask = o_cur + C, o_z = o_mask + K, o_depth = o_z + K,
-            o_dot = o_depth + 1, o_ang = o_dot + K, o_ncur = o_ang + K, o_nsrc = o_ncur + 3,
-            o_comb = o_nsrc + 3 * K, o_r = o_comb + K, o_t = o_r + K;
+  const MetaLayout o(K, C);
   const Centre ctr(s.W, s.H);
   const int tiles_per_plane = (HW + BT - 1) / BT;
   const long long n_tiles = (long long)s.B * s.D * tiles_per_plane;
@@ -240,49 +209,8 @@ mlp_backward_kernel(srcv_shape s, BwdDims m, const float* __restrict__ cur,
     for (int it = tid; it < BT * K; it += BNT) {
       const int r = it % BT, k = it / BT;
       const int p = min(p0 + r, HW - 1);
-      const float pxc = (float)(p % s.W) + 0.5f, pyc = (float)(p / s.W) + 0.5f;
-      const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p)
-                                   : __ldg(planes + b * s.D + d);
-      const ViewParams& vp = views[b * K + k];
-      Sample sm;
-      project_sample(vp, ctr, s.W, s.H, pxc, pyc, dval, sm);
-      const float* sp = src + ((size_t)(b * K + k) * C) * HW + (sm.tp.y0 * s.W + sm.tp.x0);
-      const float* cp = cur + (size_t)b * C * HW + p;
-      float dot = 0.f;
-      for (int c = 0; c < C; ++c) {
-        const float v = gather4(sp + (size_t)c * HW, s.W, sm);
-        sX[(k * C + c) * BTP + r] = v;
-        dot = fmaf(v, __ldg(cp + (size_t)c * HW), dot);
-      }
-      sX[(o_mask + k) * BTP + r] = sm.mk;
-      sX[(o_z + k) * BTP + r] = sm.zp;
-      sX[(o_dot + k) * BTP + r] = dot * sm.mk;
-      const float rx = fmaf(fp.invK[0], pxc, fmaf(fp.invK[1], pyc, fp.invK[2]));
-      const float ry = fmaf(fp.invK[3], pxc, fmaf(fp.invK[4], pyc, fp.invK[5]));
-      const float rz = fmaf(fp.invK[6], pxc, fmaf(fp.invK[7], pyc, fp.invK[8]));
-      const float X = dval * rx, Y = dval * ry, Z = dval * rz;
-      const float nc = fmaxf(sqrtf(fmaf(X, X, fmaf(Y, Y, Z * Z))), kEpsNorm);
-      const float cx = X / nc, cy = Y / nc, cz = Z / nc;
-      const float sx0 = X - vp.centre[0], sy0 = Y - vp.centre[1], sz0 = Z - vp.centre[2];
-      const float ns = fmaxf(sqrtf(fmaf(sx0, sx0, fmaf(sy0, sy0, sz0 * sz0))), kEpsNorm);
-      const float sx = sx0 / ns, sy = sy0 / ns, sz = sz0 / ns;
-      const float n1 = fmaxf(sqrtf(fmaf(cx, cx, fmaf(cy, cy, cz * cz))), kEpsCos);
-      const float n2 = fmaxf(sqrtf(fmaf(sx, sx, fmaf(sy, sy, sz * sz))), kEpsCos);
-      sX[(o_ang + k) * BTP + r] = fmaf(cx / n1, sx / n2, fmaf(cy / n1, sy / n2, (cz / n1) * (sz / n2)));
-      sX[(o_nsrc + 3 * k + 0) * BTP + r] = sx;
-      sX[(o_nsrc + 3 * k + 1) * BTP + r] = sy;
-      sX[(o_nsrc + 3 * k + 2) * BTP + r] = sz;
-      sX[(o_comb + k) * BTP + r] = vp.comb;
-      sX[(o_r + k) * BTP + r] = vp.rmeas;
-      sX[(o_t + k) * BTP + r] = vp.tmeas;
-      if (k == 0) {
-        for (int c = 0; c < C; ++c) sX[(o_cur + c) * BTP + r] = __ldg(cp + (size_t)c * HW);
-        sX[o_depth * BTP + r] = dval;
-        sX[(o_ncur + 0) * BTP + r] = cx;
-        sX[(o_ncur + 1) * BTP + r] = cy;
-        sX[(o_ncur + 2) * BTP + r] = cz;
-        for (int f = m.F; f < Fp; ++f) sX[f * BTP + r] = 0.f;
-      }
+      metadata_row(sX, BTP, r, m.F, Fp, o, s, cur, src, views[b * K + k], fp, b, k, p,
+                   plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p));
     }
     __syncthreads();
 
@@ -378,13 +306,11 @@ mlp_backward_kernel(srcv_shape s, BwdDims m, const float* __restrict__ cur,
       const int p = p0 + r;
       if (p >= HW) continue;
       const float pxc = (float)(p % s.W) + 0.5f, pyc = (float)(p / s.W) + 0.5f;
-      const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p)
-                                   : __ldg(planes + b * s.D + d);
-      Sample sm;
-      project_sample(views[b * K + k], ctr, s.W, s.H, pxc, pyc, dval, sm);
+      const Sample sm = project_sample(views[b * K + k].a0, ctr, s.W, s.H, pxc - ctr.half_w, pyc - ctr.half_h,
+                                       plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p));
       const size_t off = ((size_t)(b * K + k) * C) * HW + (sm.tp.y0 * s.W + sm.tp.x0);
       const float* cp = cur + (size_t)b * C * HW + p;
-      const float gdot = sm.mk * sX[(o_dot + k) * BTP + r];     // dL/d(dot_k) through the mask
+      const float gdot = sm.mk * sX[(o.dot + k) * BTP + r];     // dL/d(dot_k) through the mask
       for (int c = 0; c < C; ++c) {
         // dL/dwarped_kc = direct channel + via the dot product (:691-695)
         const float gw = fmaf(gdot, __ldg(cp + (size_t)c * HW), sX[(k * C + c) * BTP + r]);
@@ -397,14 +323,14 @@ mlp_backward_kernel(srcv_shape s, BwdDims m, const float* __restrict__ cur,
         }
         if (gdot != 0.f) {
           const float v = gather4(src + off + (size_t)c * HW, s.W, sm);
-          atomicAdd(&sX[(o_cur + c) * BTP + r], gdot * v);      // dL/dcur via the dot product
+          atomicAdd(&sX[(o.cur + c) * BTP + r], gdot * v);      // dL/dcur via the dot product
         }
       }
     }
     __syncthreads();
     for (int it = tid; it < BT * C; it += BNT) {
       const int r = it % BT, c = it / BT;
-      const float v = sX[(o_cur + c) * BTP + r];
+      const float v = sX[(o.cur + c) * BTP + r];
       if (p0 + r < HW && v != 0.f) atomicAdd(gcur + ((size_t)b * C + c) * HW + p0 + r, v);
     }
     __syncthreads();   // the next tile rewrites every shared buffer
@@ -417,7 +343,7 @@ size_t bwd_smem_bytes(int Fp) {
 
 BwdDims make_bwd_dims(const srcv_shape& s, const srcv_mlp_weights& w) {
   BwdDims m;
-  m.F = s.C * (s.K + 1) + 10 * s.K + 4;
+  m.F = mlp_features(s.K, s.C);
   m.Fp = padded_features(m.F);
   m.H1 = w.hidden1;
   m.H2 = w.hidden2;
@@ -427,8 +353,7 @@ BwdDims make_bwd_dims(const srcv_shape& s, const srcv_mlp_weights& w) {
 }  // namespace
 
 bool mlp_backward_supported(const srcv_shape& s, const srcv_mlp_weights& w) {
-  const int F = s.C * (s.K + 1) + 10 * s.K + 4;
-  return F <= BFMAX && w.hidden1 >= 1 && w.hidden1 <= BN && w.hidden2 >= 1 && w.hidden2 <= BN;
+  return mlp_features(s.K, s.C) <= BFMAX && w.hidden1 >= 1 && w.hidden1 <= BN && w.hidden2 >= 1 && w.hidden2 <= BN;
 }
 
 size_t mlp_backward_extra_bytes(const srcv_shape& s, const srcv_mlp_weights& w) {

@@ -36,7 +36,7 @@ struct MlpDims {
 
 __host__ __device__ inline MlpDims make_dims(int K, int C, int H1, int H2) {
   MlpDims m;
-  m.F = C * (K + 1) + 10 * K + 4;
+  m.F = mlp_features(K, C);
   m.Fp = (m.F + KC - 1) / KC * KC;
   m.H1 = H1; m.H2 = H2;
   m.H1p = (H1 + KC - 1) / KC * KC;
@@ -115,9 +115,7 @@ mlp_generic_kernel(srcv_shape s, MlpDims m, const float* __restrict__ cur,
   const int p0 = blockIdx.x * TM;
   const bool want_mask = (mask_out != nullptr) && (d == s.D - 1);
 
-  const int o_cur = K * C, o_mask = o_cur + C, o_z = o_mask + K, o_depth = o_z + K,
-            o_dot = o_depth + 1, o_ang = o_dot + K, o_ncur = o_ang + K, o_nsrc = o_ncur + 3,
-            o_comb = o_nsrc + 3 * K, o_r = o_comb + K, o_t = o_r + K;
+  const MetaLayout o(K, C);
   const Centre ctr(s.W, s.H);
   const FrameParams fp = frames[b];
 
@@ -128,69 +126,12 @@ mlp_generic_kernel(srcv_shape s, MlpDims m, const float* __restrict__ cur,
   for (int it = tid; it < TM * K; it += NT) {
     const int r = it % TM, k = it / TM;
     const int p = min(p0 + r, HW - 1);
-    const float pxc = (float)(p % s.W) + 0.5f, pyc = (float)(p / s.W) + 0.5f;
-    const float dval = PER_PIXEL ? __ldg(planes + ((size_t)b * s.D + d) * HW + p)
-                                 : __ldg(planes + b * s.D + d);
-    const ViewParams& vp = views[b * K + k];
-    float ax, ay, az, px, py, zp;
-    homography_point(vp.a0, pxc - ctr.half_w, pyc - ctr.half_h, ax, ay, az);
-    project_point(dval, ax, ay, az, vp.t[0], vp.t[1], vp.t[2], px, py, zp);
-    Taps tp;
-    bilinear_taps(px, py, s.W, s.H, ctr, tp);
-    const float w00 = (1.0f - tp.fx) * (1.0f - tp.fy), w01 = tp.fx * (1.0f - tp.fy);
-    const float w10 = (1.0f - tp.fx) * tp.fy, w11 = tp.fx * tp.fy;
-    const float mk = zp > 0.0f ? 1.0f : 0.0f;
-    // warped features + per-view dot (features are sampled even behind the camera,
-    // reference modules/cost_volume.py:590-623: only the dot is masked)
-    const float* sp = src + ((size_t)(b * K + k) * C) * HW + (tp.y0 * s.W + tp.x0);
-    const float* cp = cur + (size_t)b * C * HW + p;
-    float dot = 0.f;
-    for (int c = 0; c < C; ++c) {
-      const float* q = sp + (size_t)c * HW;
-      float v = 0.f;
-      if (tp.valid & 1u) v = w00 * __ldg(q);
-      if (tp.valid & 2u) v = fmaf(w01, __ldg(q + 1), v);
-      if (tp.valid & 4u) v = fmaf(w10, __ldg(q + s.W), v);
-      if (tp.valid & 8u) v = fmaf(w11, __ldg(q + s.W + 1), v);
-      sA[(k * C + c) * TM + r] = v;
-      dot = fmaf(v, __ldg(cp + (size_t)c * HW), dot);
-    }
-    sA[(o_mask + k) * TM + r] = mk;
-    sA[(o_z + k) * TM + r] = zp;
-    sA[(o_dot + k) * TM + r] = dot * mk;
-    // rays: X = d * (invK3 p); n_cur = X/|X|; n_src = (X - centre_k)/|.|
-    const float rx = fmaf(fp.invK[0], pxc, fmaf(fp.invK[1], pyc, fp.invK[2]));
-    const float ry = fmaf(fp.invK[3], pxc, fmaf(fp.invK[4], pyc, fp.invK[5]));
-    const float rz = fmaf(fp.invK[6], pxc, fmaf(fp.invK[7], pyc, fp.invK[8]));
-    const float X = dval * rx, Y = dval * ry, Z = dval * rz;
-    const float nc = fmaxf(sqrtf(fmaf(X, X, fmaf(Y, Y, Z * Z))), kEpsNorm);
-    const float cx = X / nc, cy = Y / nc, cz = Z / nc;
-    const float sx0 = X - vp.centre[0], sy0 = Y - vp.centre[1], sz0 = Z - vp.centre[2];
-    const float ns = fmaxf(sqrtf(fmaf(sx0, sx0, fmaf(sy0, sy0, sz0 * sz0))), kEpsNorm);
-    const float sx = sx0 / ns, sy = sy0 / ns, sz = sz0 / ns;
-    // cosine_similarity(eps=1e-5) of the two (already unit) rays
-    const float n1 = fmaxf(sqrtf(fmaf(cx, cx, fmaf(cy, cy, cz * cz))), kEpsCos);
-    const float n2 = fmaxf(sqrtf(fmaf(sx, sx, fmaf(sy, sy, sz * sz))), kEpsCos);
-    const float ang = fmaf(cx / n1, sx / n2, fmaf(cy / n1, sy / n2, (cz / n1) * (sz / n2)));
-    sA[(o_ang + k) * TM + r] = ang;
-    sA[(o_nsrc + 3 * k + 0) * TM + r] = sx;
-    sA[(o_nsrc + 3 * k + 1) * TM + r] = sy;
-    sA[(o_nsrc + 3 * k + 2) * TM + r] = sz;
-    sA[(o_comb + k) * TM + r] = vp.comb;
-    sA[(o_r + k) * TM + r] = vp.rmeas;
-    sA[(o_t + k) * TM + r] = vp.tmeas;
-    if (k == 0) {
-      for (int c = 0; c < C; ++c) sA[(o_cur + c) * TM + r] = __ldg(cp + (size_t)c * HW);
-      sA[o_depth * TM + r] = dval;
-      sA[(o_ncur + 0) * TM + r] = cx;
-      sA[(o_ncur + 1) * TM + r] = cy;
-      sA[(o_ncur + 2) * TM + r] = cz;
-      for (int f = m.F; f < m.rows; ++f) sA[f * TM + r] = 0.f;
-    }
+    const Sample sm = metadata_row(sA, TM, r, m.F, m.rows, o, s, cur, src, views[b * K + k], fp, b, k, p,
+                                   plane_depth<PER_PIXEL>(planes, b, s.D, d, HW, p));
     if (want_mask) {
       int bits = 0;
-      if (zp > 0.0f) bits |= 1;
-      if (in_mask_bounds(px, py, s.W, s.H, ctr)) bits |= 2;
+      if (sm.zp > 0.0f) bits |= 1;
+      if (in_mask_bounds(sm.px, sm.py, s.W, s.H, ctr)) bits |= 2;
       if (bits) atomicOr(&sFlag[r], bits);
     }
   }
