@@ -418,6 +418,54 @@ int32_t srcv_mvloss_backward_f32(const srcv_mvloss_args* args, const float* grad
                                  float* grad_depth_pred, const void* workspace, size_t workspace_bytes,
                                  void* stream);
 
+/* ---- depth metrics (evaluation and training logs) ------------------------------------ *
+ * Replaces compute_depth_metrics_batched and compute_depth_metrics of the reference
+ * (utils/metrics_utils.py:7-120) together with the resampling test.py:282-299 runs before them
+ * (F.interpolate of the prediction to the ground-truth size, then gt > 0.5).  DESIGN §4.12.
+ *   gt     DEVICE (B,H,W) fp32 ground truth          pred  DEVICE (B,Hp,Wp) fp32 prediction
+ *   valid  DEVICE (B,H,W) uint8 (0 = invalid), read when valid_source == SRCV_METRICS_VALID_MASK
+ *   (each may be NULL when it holds no element: H*W == 0 gives NaN metrics and zero counts)
+ * Per pixel, with the prediction v sampled at the ground-truth pixel (PyTorch's rules,
+ * align_corners=False; a same-size nearest or bilinear resampling is the identity):
+ *   thresh = max(gt/v, v/gt) (NaN-propagating); a_t counts thresh < t for the fp32 constants
+ *   1.05, 1.10, 1.25, 1.25^2, 1.25^3; the terms |gt-v|, |gt-v|/gt, (gt-v)^2/gt, (gt-v)^2 and
+ *   (log gt - log v)^2 are fp32 ops in the reference's order.
+ * Sums are fp64, counts are integers, and each metric is the fp32 rounding of the fp64 formula:
+ *   metrics (B,12) f32 out: abs_diff, abs_rel, sq_rel, rmse, rmse_log, a5, a10, a25, a0 (= a10),
+ *                  a1 (= a25), a2, a3 — the a-values are a_count / valid_count, times 100 in
+ *                  fp32 when mult_a; rmse and rmse_log are sqrt of the mean;
+ *   valid_counts (B) int64 out; upsampled (B,H,W) f32 out = the resampled prediction, or NULL.
+ * SRCV_METRICS_BATCHED: each continuous metric is the mean of its non-NaN terms (nanmean);
+ * SRCV_METRICS_FLAT: plain means, NaN if any term is NaN.  A frame without valid pixels gives NaN.
+ * Two launches (per-CTA partials, then one CTA per frame summing them in a fixed order): no
+ * atomics, no host synchronisation, bit-identical on every run.  At most 2^30 pixels per frame
+ * (H*W and Hp*Wp), B <= 65535.  Workspace: 128 bytes per 1024 ground-truth pixels per frame.     */
+typedef enum srcv_resample_mode {
+  SRCV_RESAMPLE_IDENTITY = 0, /* Hp == H, Wp == W                         */
+  SRCV_RESAMPLE_NEAREST = 1,  /* src = min(floor(dst * fp32(in/out)), in-1) */
+  SRCV_RESAMPLE_BILINEAR = 2  /* src = max(0, fp32(in/out) (dst + 0.5) - 0.5) */
+} srcv_resample_mode;
+typedef enum srcv_metrics_nan_mode { SRCV_METRICS_BATCHED = 0, SRCV_METRICS_FLAT = 1 } srcv_metrics_nan_mode;
+typedef enum srcv_metrics_valid_source {
+  SRCV_METRICS_VALID_MASK = 0,      /* valid[p] != 0                 */
+  SRCV_METRICS_VALID_MIN_DEPTH = 1, /* gt > min_valid_depth, in fp32 */
+  SRCV_METRICS_VALID_ALL = 2        /* every pixel                   */
+} srcv_metrics_valid_source;
+typedef struct srcv_metrics_args {
+  const float* gt;
+  const float* pred;
+  const uint8_t* valid;
+  float min_valid_depth;
+  int32_t B, H, W, Hp, Wp;
+  int32_t resample;      /* srcv_resample_mode        */
+  int32_t nan_mode;      /* srcv_metrics_nan_mode     */
+  int32_t valid_source;  /* srcv_metrics_valid_source */
+  int32_t mult_a;
+} srcv_metrics_args;
+size_t srcv_metrics_workspace_bytes(const srcv_metrics_args* args);
+int32_t srcv_depth_metrics_f32(const srcv_metrics_args* args, float* metrics, int64_t* valid_counts, float* upsampled,
+                               void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- tuning / introspection ------------------------------------------- *
  * Selects the kernel variant used by the two forward calls on this thread's
  * next invocations (process-global).  0 = automatic choice.  Used by the tests

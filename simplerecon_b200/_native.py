@@ -87,6 +87,16 @@ class MvLossArgs(C.Structure):
                                    "src_cam_T_world")] + [(n, C.c_int32) for n in ("B", "K", "H", "W")]
 
 
+RESAMPLE_IDENTITY, RESAMPLE_NEAREST, RESAMPLE_BILINEAR = 0, 1, 2
+METRICS_BATCHED, METRICS_FLAT = 0, 1
+METRICS_VALID_MASK, METRICS_VALID_MIN_DEPTH, METRICS_VALID_ALL = 0, 1, 2
+
+
+class MetricsArgs(C.Structure):
+    _fields_ = [("gt", _fp), ("pred", _fp), ("valid", _fp), ("min_valid_depth", C.c_float)] + \
+        [(n, C.c_int32) for n in ("B", "H", "W", "Hp", "Wp", "resample", "nan_mode", "valid_source", "mult_a")]
+
+
 # every symbol include/srcv_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "srcv_abi_version": (C.c_int32, []),
@@ -133,6 +143,8 @@ SYMBOLS = {
     "srcv_mvloss_workspace_bytes": (C.c_size_t, [C.POINTER(MvLossArgs)]),
     "srcv_mvloss_forward_f32": (C.c_int32, [C.POINTER(MvLossArgs), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_mvloss_backward_f32": (C.c_int32, [C.POINTER(MvLossArgs), _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_metrics_workspace_bytes": (C.c_size_t, [C.POINTER(MetricsArgs)]),
+    "srcv_depth_metrics_f32": (C.c_int32, [C.POINTER(MetricsArgs), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_set_variant": (C.c_int32, [C.c_int32]),
     "srcv_last_variant": (C.c_char_p, []),
     "srcv_launch_count": (C.c_uint64, []),

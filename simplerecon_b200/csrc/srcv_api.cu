@@ -616,6 +616,49 @@ int32_t srcv_mvloss_backward_f32(const srcv_mvloss_args* a, const float* grad_lo
   return SRCV_OK;
 }
 
+static bool metrics_dims_ok(const srcv_metrics_args* a) {
+  return a->B > 0 && a->H >= 0 && a->W >= 0 && a->Hp >= 0 && a->Wp >= 0 && metrics_shape_supported(*a);
+}
+
+size_t srcv_metrics_workspace_bytes(const srcv_metrics_args* a) {
+  if (!a || !metrics_dims_ok(a)) return 0;
+  return metrics_workspace_bytes(*a);
+}
+
+int32_t srcv_depth_metrics_f32(const srcv_metrics_args* a, float* metrics, int64_t* valid_counts, float* upsampled,
+                               void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!a) return fail(SRCV_ERR_NULL, "metrics arguments are NULL");
+  const bool any_gt = (long long)a->H * a->W > 0;     // an empty input (nothing to read) may pass NULL
+  if ((any_gt && !a->gt) || ((long long)a->Hp * a->Wp > 0 && !a->pred)) return fail(SRCV_ERR_NULL, "gt / pred is NULL");
+  if (!metrics || !valid_counts) return fail(SRCV_ERR_NULL, "metrics / valid_counts output is NULL");
+  if (any_gt && a->valid_source == SRCV_METRICS_VALID_MASK && !a->valid)
+    return fail(SRCV_ERR_NULL, "valid mask is NULL");
+  if (a->valid_source < SRCV_METRICS_VALID_MASK || a->valid_source > SRCV_METRICS_VALID_ALL)
+    return fail(SRCV_ERR_UNSUPPORTED, "unknown valid_source %d", a->valid_source);
+  if (a->nan_mode != SRCV_METRICS_BATCHED && a->nan_mode != SRCV_METRICS_FLAT)
+    return fail(SRCV_ERR_UNSUPPORTED, "unknown nan_mode %d", a->nan_mode);
+  if (a->resample < SRCV_RESAMPLE_IDENTITY || a->resample > SRCV_RESAMPLE_BILINEAR)
+    return fail(SRCV_ERR_UNSUPPORTED, "unknown resample mode %d", a->resample);
+  if (!metrics_dims_ok(a))
+    return fail(SRCV_ERR_SHAPE, "bad metrics shape B=%d H=%d W=%d Hp=%d Wp=%d (B in [1, 65535], at most 2^30 pixels per frame)",
+                a->B, a->H, a->W, a->Hp, a->Wp);
+  srcv_metrics_args run = *a;
+  if (a->Hp == a->H && a->Wp == a->W) {
+    run.resample = SRCV_RESAMPLE_IDENTITY;        // PyTorch copies a same-size input in both modes
+  } else if (a->resample == SRCV_RESAMPLE_IDENTITY) {
+    return fail(SRCV_ERR_SHAPE, "identity resampling needs Hp == H and Wp == W (got %dx%d -> %dx%d)", a->Hp, a->Wp,
+                a->H, a->W);
+  } else if (a->Hp < 1 || a->Wp < 1) {
+    return fail(SRCV_ERR_SHAPE, "cannot resample an empty prediction (%dx%d) to %dx%d", a->Hp, a->Wp, a->H, a->W);
+  }
+  if (int32_t e = check_workspace(workspace, workspace_bytes, metrics_workspace_bytes(*a))) return e;
+  g_last_variant.store("depth_metrics_f32");
+  cudaError_t err = launch_metrics(run, metrics, reinterpret_cast<long long*>(valid_counts), upsampled, workspace,
+                                   static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "depth_metrics");
+  return SRCV_OK;
+}
+
 int32_t srcv_tc_selftest_f32(const float* A, const float* Wm, int32_t Kp, float* D, void* scratch,
                              void* stream) {
   if (!A || !Wm || !D || !scratch) return fail(SRCV_ERR_NULL, "selftest pointer is NULL");

@@ -128,6 +128,13 @@ cudaError_t launch_mvloss_forward(const srcv_mvloss_args& a, float* loss, uint8_
 cudaError_t launch_mvloss_backward(const srcv_mvloss_args& a, const float* grad_loss, float* grad_pred,
                                    const void* workspace, cudaStream_t stream);
 
+// depth metrics (csrc/srcv_metrics.cuh, compiled in the srcv_mvloss.cu unit)
+constexpr long long kMetricsMaxPixels = 1ll << 30;   // per frame, so that 32-bit pixel indices never overflow
+bool metrics_shape_supported(const srcv_metrics_args& a);
+size_t metrics_workspace_bytes(const srcv_metrics_args& a);
+cudaError_t launch_metrics(const srcv_metrics_args& a, float* metrics, long long* valid_counts, float* upsampled,
+                           void* workspace, cudaStream_t stream);
+
 // argmax over planes -> plane depth (used by variants that do not fuse it)
 cudaError_t launch_argmax(const srcv_shape& s, const float* cost, const float* planes,
                           bool per_pixel, float* lowest, cudaStream_t stream);

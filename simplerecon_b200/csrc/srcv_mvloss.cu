@@ -222,3 +222,5 @@ cudaError_t launch_mvloss_backward(const srcv_mvloss_args& a, const float* grad_
 }
 
 }  // namespace srcv
+
+#include "srcv_metrics.cuh"   // depth metrics (DESIGN §4.12), compiled in this unit

@@ -12,6 +12,10 @@ the names ``tools.fusers_helper`` bound at import (tools/fusers_helper.py:8) if 
 imported.  ``install(fusion=True, fuse_color=True)`` also wraps ``tools.fusers_helper.get_fuser`` so that
 ``--depth_fuser ours --fuse_color`` gets a ``fusers.ColorFuser`` (colour fused on the GPU) instead of the
 reference's warning and a colourless ``OurFuser``; every other option goes to the original.
+``install(metrics=True)`` swaps ``compute_depth_metrics`` / ``compute_depth_metrics_batched`` of
+``utils.metrics_utils`` (and the name ``experiment_modules.depth_model`` binds at import, :16, if it was
+already imported) for wrappers that run CUDA tensors through the metrics kernel and hand anything else to
+the saved originals, so CPU callers of that utility module keep working.
 ``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
@@ -19,14 +23,18 @@ from __future__ import annotations
 import importlib
 import sys
 
+import torch
+
 _NAMES = ("CostVolumeManager", "FeatureVolumeManager", "FastFeatureVolumeManager")
 _saved: dict = {}
 
 
-def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False) -> list[str]:
+def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False,
+            metrics: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
-    with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``."""
+    with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``,
+    with ``metrics=True`` also as ``utils.metrics_utils``."""
     if fuse_color and not fusion:
         raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
     from . import cost_volume as ours
@@ -65,6 +73,16 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
         if fuse_color:
             _saved.setdefault((fh.__name__, "get_fuser"), fh.get_fuser)
             fh.get_fuser = _color_get_fuser(_saved[(fh.__name__, "get_fuser")], fh)
+    if metrics:
+        from . import metrics as ours_metrics
+        mu = importlib.import_module("utils.metrics_utils")
+        for mod in [mu] + ([dm] if dm is not None else []):       # depth_model binds compute_depth_metrics (:16)
+            for n in ("compute_depth_metrics", "compute_depth_metrics_batched"):
+                if hasattr(mod, n):
+                    _saved.setdefault((mod.__name__, n), getattr(mod, n))
+                    setattr(mod, n, _cuda_or_original(getattr(ours_metrics, n), _saved[(mod.__name__, n)]))
+            if mod.__name__ not in patched:
+                patched.append(mod.__name__)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched
@@ -84,6 +102,18 @@ def _color_get_fuser(original, fh):
                           max_fusion_depth=opts.fusion_max_depth, fuse_color=True)
     get_fuser.__wrapped__ = original
     return get_fuser
+
+
+def _cuda_or_original(fast, original):
+    """``fast`` for CUDA ground truth, ``original`` for anything else (CPU callers of the utility module)."""
+    def metrics_fn(gt, *args, **kwargs):
+        if torch.is_tensor(gt) and gt.is_cuda:
+            return fast(gt, *args, **kwargs)
+        return original(gt, *args, **kwargs)
+    metrics_fn.__name__ = original.__name__
+    metrics_fn.__doc__ = fast.__doc__
+    metrics_fn.__wrapped__ = original
+    return metrics_fn
 
 
 def uninstall() -> None:
