@@ -466,6 +466,51 @@ size_t srcv_metrics_workspace_bytes(const srcv_metrics_args* args);
 int32_t srcv_depth_metrics_f32(const srcv_metrics_args* args, float* metrics, int64_t* valid_counts, float* upsampled,
                                void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- surface normals from depth (training loss, Equation 4) --------------------------- *
+ * Replaces NormalGenerator.forward of the reference (utils/geometry_utils.py:92-133; called twice
+ * per training step, experiment_modules/depth_model.py:526, :530).  DESIGN §4.13.  Per pixel:
+ *   S = the separable Gaussian blur of depth (x pass, then y pass, cross-correlations with `taps`,
+ *       PyTorch 'reflect' padding);  P = S * invK[:3,:3] (x + .5, y + .5, 1);
+ *   Gx, Gy = Sobel of P, normalised (1/8), replicate padding (a tap outside the map reads P of the
+ *       clamped pixel);  normal = c / max(|c|, 1e-12), c = Gx x Gy.
+ * A non-finite depth anywhere in the pixel's (k + 2) x (k + 2) window (after the reflect and clamp
+ * maps) makes all three components NaN.  All pointers DEVICE memory, dense fp32:
+ *   depth (B,1,H,W)   invK (B,4,4)   taps (k) (the caller computes them, kornia's gaussian(k, sigma))
+ *   normals (B,3,H,W) out
+ * backward: grad_depth (B,1,H,W) out from grad_normals (B,3,H,W).  Pixels whose window holds a
+ *   non-finite depth pass no gradient.  Workspace: srcv_normals_workspace_bytes (24 bytes per pixel),
+ *   scratch only (nothing is kept between calls).
+ * Limits (SRCV_ERR_SHAPE): k odd in [1, 15]; min(H, W) > k/2 (the reflect padding); 1 <= B <= 65535;
+ * 6 B H W < 2^31 (32-bit element indices).  One forward launch, two backward launches; gather form,
+ * no atomics: bit-identical on every run.                                                         */
+typedef struct srcv_normals_args {
+  const float* depth;
+  const float* invK;
+  const float* taps;
+  int32_t B, H, W, k;
+} srcv_normals_args;
+size_t srcv_normals_workspace_bytes(const srcv_normals_args* args);
+int32_t srcv_normals_forward_f32(const srcv_normals_args* args, float* normals, void* stream);
+int32_t srcv_normals_backward_f32(const srcv_normals_args* args, const float* grad_normals, float* grad_depth,
+                                  void* workspace, size_t workspace_bytes, void* stream);
+
+/* ---- normals loss ----------------------------------------------------------------------- *
+ * Replaces NormalsLoss.forward of the reference (losses.py:57-77; depth_model.py:475): the mean over
+ * the pixels whose six components (both normals) are finite of 0.5 (1 - pred . gt), fp32 terms, fp64
+ * sum, exact count.  No such pixel: the loss is NaN and the gradients are zero.
+ *   normals_gt, normals_pred DEVICE (B,3,H,W) fp32     loss DEVICE (1 float) out
+ * backward: grad_pred = -0.5 gt (grad_loss[0] / count) at masked pixels and 0 elsewhere; grad_gt the
+ *   same with pred (grad_gt may be NULL).  `workspace` must be the one the forward call on the same
+ *   inputs filled: it keeps the count, so nothing goes through the host.
+ * Limits: B, H, W >= 1, 3 B H W < 2^31.  Two forward launches (per-CTA partials, a fixed-order
+ * finalize), one backward launch; bit-identical on every run.                                     */
+size_t srcv_normals_loss_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int32_t srcv_normals_loss_forward_f32(const float* normals_gt, const float* normals_pred, int32_t B, int32_t H,
+                                      int32_t W, float* loss, void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_normals_loss_backward_f32(const float* normals_gt, const float* normals_pred, int32_t B, int32_t H,
+                                       int32_t W, const float* grad_loss, float* grad_pred, float* grad_gt,
+                                       const void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- tuning / introspection ------------------------------------------- *
  * Selects the kernel variant used by the two forward calls on this thread's
  * next invocations (process-global).  0 = automatic choice.  Used by the tests

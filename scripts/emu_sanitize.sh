@@ -2,11 +2,22 @@
 # Runs tests/test_emu_kernels.py (the SIMT kernels compiled for the host, tests/emu) under
 # ThreadSanitizer — a missing __syncthreads() shows up as a data race on the emulated shared
 # memory — and AddressSanitizer — out-of-bounds global / shared accesses.  CPU only.
-#   scripts/emu_sanitize.sh [thread|address ...]   (default: both)   report -> stdout
+#   scripts/emu_sanitize.sh [thread|address ...] [tests/test_emu_<x>.py ...]
+#   (default: both sanitizers, tests/test_emu_kernels.py)   report -> stdout
 set -u
 cd "$(dirname "$0")/.."
 CXX=/usr/bin/g++
-for san in "${@:-thread address}"; do
+sans=()
+tests=()
+for a in "$@"; do
+  case $a in
+    *.py|*::*) tests+=("$a") ;;
+    *) sans+=("$a") ;;
+  esac
+done
+[ ${#sans[@]} -eq 0 ] && sans=("thread address")
+[ ${#tests[@]} -eq 0 ] && tests=(tests/test_emu_kernels.py)
+for san in "${sans[@]}"; do
   for s in $san; do
     lib=$(python -c "from tests import emu; print(emu.build(sanitize='$s'))") || exit 1
     case $s in
@@ -16,7 +27,7 @@ for san in "${@:-thread address}"; do
     esac
     echo "== $s sanitizer: $lib"
     log=$(mktemp)
-    env LD_PRELOAD="$rt" $opts SRCV_EMU_LIB="$lib" python -m pytest tests/test_emu_kernels.py -q -x -s -p no:cacheprovider >"$log" 2>&1
+    env LD_PRELOAD="$rt" $opts SRCV_EMU_LIB="$lib" python -m pytest "${tests[@]}" -q -x -s -p no:cacheprovider >"$log" 2>&1
     rc=$?
     tail -n 3 "$log"
     echo "pytest exit code: $rc"

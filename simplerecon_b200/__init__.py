@@ -24,3 +24,4 @@ from .fusers import ColorFuser  # noqa: E402,F401  (OurFuser with colour, DESIGN
 from . import point_cloud_fusion  # noqa: E402,F401  (reference tools/torch_point_cloud_fusion.py)
 from .losses import MVDepthLoss  # noqa: E402,F401  (reference losses.py:79-208)
 from .metrics import compute_depth_metrics, compute_depth_metrics_batched, depth_metrics  # noqa: E402,F401  (reference utils/metrics_utils.py)
+from .normals import NormalGenerator, NormalsLoss  # noqa: E402,F401  (reference geometry_utils.py:92-133, losses.py:57-77)

@@ -97,6 +97,10 @@ class MetricsArgs(C.Structure):
         [(n, C.c_int32) for n in ("B", "H", "W", "Hp", "Wp", "resample", "nan_mode", "valid_source", "mult_a")]
 
 
+class NormalsArgs(C.Structure):
+    _fields_ = [("depth", _fp), ("invK", _fp), ("taps", _fp)] + [(n, C.c_int32) for n in ("B", "H", "W", "k")]
+
+
 # every symbol include/srcv_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "srcv_abi_version": (C.c_int32, []),
@@ -145,6 +149,14 @@ SYMBOLS = {
     "srcv_mvloss_backward_f32": (C.c_int32, [C.POINTER(MvLossArgs), _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_metrics_workspace_bytes": (C.c_size_t, [C.POINTER(MetricsArgs)]),
     "srcv_depth_metrics_f32": (C.c_int32, [C.POINTER(MetricsArgs), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_normals_workspace_bytes": (C.c_size_t, [C.POINTER(NormalsArgs)]),
+    "srcv_normals_forward_f32": (C.c_int32, [C.POINTER(NormalsArgs), _fp, _fp]),
+    "srcv_normals_backward_f32": (C.c_int32, [C.POINTER(NormalsArgs), _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_normals_loss_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32]),
+    "srcv_normals_loss_forward_f32": (C.c_int32, [_fp, _fp, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, C.c_size_t,
+                                                  _fp]),
+    "srcv_normals_loss_backward_f32": (C.c_int32, [_fp, _fp, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp,
+                                                   C.c_size_t, _fp]),
     "srcv_set_variant": (C.c_int32, [C.c_int32]),
     "srcv_last_variant": (C.c_char_p, []),
     "srcv_launch_count": (C.c_uint64, []),

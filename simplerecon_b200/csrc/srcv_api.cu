@@ -659,6 +659,83 @@ int32_t srcv_depth_metrics_f32(const srcv_metrics_args* a, float* metrics, int64
   return SRCV_OK;
 }
 
+static bool normals_dims_ok(const srcv_normals_args* a) {
+  return a->B >= 1 && a->B <= 65535 && a->H >= 1 && a->W >= 1 && (a->k & 1) && a->k >= 1 &&
+         a->k <= kNormalsMaxKernel && (a->H < a->W ? a->H : a->W) > a->k / 2 &&
+         6ll * a->B * a->H * a->W < (1ll << 31);
+}
+
+static int32_t check_normals(const srcv_normals_args* a) {
+  if (!a) return fail(SRCV_ERR_NULL, "normals arguments are NULL");
+  if (!a->depth || !a->invK || !a->taps) return fail(SRCV_ERR_NULL, "depth / invK / taps is NULL");
+  if (!normals_dims_ok(a))
+    return fail(SRCV_ERR_SHAPE, "bad normals shape B=%d H=%d W=%d k=%d (k odd in [1, %d], min(H, W) > k/2, "
+                "B <= 65535, 6 B H W < 2^31)", a->B, a->H, a->W, a->k, kNormalsMaxKernel);
+  return SRCV_OK;
+}
+
+size_t srcv_normals_workspace_bytes(const srcv_normals_args* a) {
+  if (!a || !normals_dims_ok(a)) return 0;
+  return normals_workspace_bytes(*a);
+}
+
+int32_t srcv_normals_forward_f32(const srcv_normals_args* a, float* normals, void* stream_) {
+  if (int32_t e = check_normals(a)) return e;
+  if (!normals) return fail(SRCV_ERR_NULL, "normals output is NULL");
+  g_last_variant.store("normals_forward_f32");
+  cudaError_t err = launch_normals_forward(*a, normals, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "normals_forward");
+  return SRCV_OK;
+}
+
+int32_t srcv_normals_backward_f32(const srcv_normals_args* a, const float* grad_normals, float* grad_depth,
+                                  void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_normals(a)) return e;
+  if (!grad_normals || !grad_depth) return fail(SRCV_ERR_NULL, "grad_normals / grad_depth is NULL");
+  if (int32_t e = check_workspace(workspace, workspace_bytes, normals_workspace_bytes(*a))) return e;
+  g_last_variant.store("normals_backward_f32");
+  cudaError_t err = launch_normals_backward(*a, grad_normals, grad_depth, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "normals_backward");
+  return SRCV_OK;
+}
+
+static bool normals_loss_dims_ok(int32_t B, int32_t H, int32_t W) {
+  return B >= 1 && H >= 1 && W >= 1 && 3ll * B * H * W < (1ll << 31);
+}
+
+size_t srcv_normals_loss_workspace_bytes(int32_t B, int32_t H, int32_t W) {
+  if (!normals_loss_dims_ok(B, H, W)) return 0;
+  return normals_loss_workspace_bytes(B, H, W);
+}
+
+int32_t srcv_normals_loss_forward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W, float* loss,
+                                      void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!gt || !pred || !loss) return fail(SRCV_ERR_NULL, "normals_gt / normals_pred / loss is NULL");
+  if (!normals_loss_dims_ok(B, H, W))
+    return fail(SRCV_ERR_SHAPE, "bad normals-loss shape B=%d H=%d W=%d (3 B H W < 2^31)", B, H, W);
+  if (int32_t e = check_workspace(workspace, workspace_bytes, normals_loss_workspace_bytes(B, H, W))) return e;
+  g_last_variant.store("normals_loss_forward_f32");
+  cudaError_t err = launch_normals_loss_forward(gt, pred, B, H, W, loss, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "normals_loss_forward");
+  return SRCV_OK;
+}
+
+int32_t srcv_normals_loss_backward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W,
+                                       const float* grad_loss, float* grad_pred, float* grad_gt,
+                                       const void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!gt || !pred || !grad_loss || !grad_pred)
+    return fail(SRCV_ERR_NULL, "normals_gt / normals_pred / grad_loss / grad_pred is NULL");
+  if (!normals_loss_dims_ok(B, H, W))
+    return fail(SRCV_ERR_SHAPE, "bad normals-loss shape B=%d H=%d W=%d (3 B H W < 2^31)", B, H, W);
+  if (int32_t e = check_workspace(const_cast<void*>(workspace), workspace_bytes, normals_loss_workspace_bytes(B, H, W)))
+    return e;
+  g_last_variant.store("normals_loss_backward_f32");
+  cudaError_t err = launch_normals_loss_backward(gt, pred, B, H, W, grad_loss, grad_pred, grad_gt, workspace,
+                                                 static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "normals_loss_backward");
+  return SRCV_OK;
+}
+
 int32_t srcv_tc_selftest_f32(const float* A, const float* Wm, int32_t Kp, float* D, void* scratch,
                              void* stream) {
   if (!A || !Wm || !D || !scratch) return fail(SRCV_ERR_NULL, "selftest pointer is NULL");

@@ -135,6 +135,19 @@ size_t metrics_workspace_bytes(const srcv_metrics_args& a);
 cudaError_t launch_metrics(const srcv_metrics_args& a, float* metrics, long long* valid_counts, float* upsampled,
                            void* workspace, cudaStream_t stream);
 
+// surface normals from depth and the normals loss (csrc/srcv_normals.cuh, compiled in the srcv_mvloss.cu unit)
+constexpr int kNormalsMaxKernel = 15;                 // largest (odd) Gaussian kernel size
+size_t normals_workspace_bytes(const srcv_normals_args& a);
+cudaError_t launch_normals_forward(const srcv_normals_args& a, float* normals, cudaStream_t stream);
+cudaError_t launch_normals_backward(const srcv_normals_args& a, const float* grad_normals, float* grad_depth,
+                                    void* workspace, cudaStream_t stream);
+size_t normals_loss_workspace_bytes(int B, int H, int W);
+cudaError_t launch_normals_loss_forward(const float* gt, const float* pred, int B, int H, int W, float* loss,
+                                        void* workspace, cudaStream_t stream);
+cudaError_t launch_normals_loss_backward(const float* gt, const float* pred, int B, int H, int W,
+                                         const float* grad_loss, float* grad_pred, float* grad_gt,
+                                         const void* workspace, cudaStream_t stream);
+
 // argmax over planes -> plane depth (used by variants that do not fuse it)
 cudaError_t launch_argmax(const srcv_shape& s, const float* cost, const float* planes,
                           bool per_pixel, float* lowest, cudaStream_t stream);

@@ -16,6 +16,9 @@ reference's warning and a colourless ``OurFuser``; every other option goes to th
 ``utils.metrics_utils`` (and the name ``experiment_modules.depth_model`` binds at import, :16, if it was
 already imported) for wrappers that run CUDA tensors through the metrics kernel and hand anything else to
 the saved originals, so CPU callers of that utility module keep working.
+``install(normals=True)`` swaps ``utils.geometry_utils.NormalGenerator`` and ``losses.NormalsLoss`` (the
+normals term of the training loss, depth_model.py:143, :156, :475) for the kernel-backed mirrors, and the
+names ``experiment_modules.depth_model`` binds at import (:7, :15) if it was already imported.
 ``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
@@ -30,11 +33,12 @@ _saved: dict = {}
 
 
 def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False,
-            metrics: bool = False) -> list[str]:
+            metrics: bool = False, normals: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
     with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``,
-    with ``metrics=True`` also as ``utils.metrics_utils``."""
+    with ``metrics=True`` also as ``utils.metrics_utils``, with ``normals=True`` also as ``losses`` and
+    ``utils.geometry_utils``."""
     if fuse_color and not fusion:
         raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
     from . import cost_volume as ours
@@ -83,6 +87,15 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
                     setattr(mod, n, _cuda_or_original(getattr(ours_metrics, n), _saved[(mod.__name__, n)]))
             if mod.__name__ not in patched:
                 patched.append(mod.__name__)
+    if normals:
+        from . import normals as ours_normals
+        for mod_name, n in (("utils.geometry_utils", "NormalGenerator"), ("losses", "NormalsLoss")):
+            for mod in [importlib.import_module(mod_name)] + ([dm] if dm is not None else []):
+                if hasattr(mod, n):
+                    _saved.setdefault((mod.__name__, n), getattr(mod, n))
+                    setattr(mod, n, getattr(ours_normals, n))
+                    if mod.__name__ not in patched:
+                        patched.append(mod.__name__)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched

@@ -316,3 +316,31 @@ def make_color_tsdf_case(seed: int = 0, frames: int = 2, voxel_size: float = 0.0
     mean = torch.tensor(IMAGENET_MEAN).view(1, 3, 1, 1)
     std = torch.tensor(IMAGENET_STD).view(1, 3, 1, 1)
     return dict(c, color=((raw - mean) / std).contiguous(), color_raw=raw.contiguous())
+
+
+def make_normals_batch(seed: int = 0, batch: int = 2, height: int = 48, width: int = 64, holes: bool = True,
+                       pred_noise: float = 0.03) -> dict:
+    """Inputs of the normals term of the training loss (reference experiment_modules/depth_model.py:526-530,
+    :475): ray-cast room depth maps with their 4x4 inverse intrinsics, and a predicted depth = ground truth x
+    exp(smooth noise) (positive and finite, as the model's head produces).  With `holes` the ground truth
+    gets what the datasets' invalid pixels look like: a NaN blob, isolated single-pixel NaNs and a
+    zero-depth patch."""
+    g = torch.Generator().manual_seed(5151 + seed)
+    sc = make_mvs_scene(seed=seed, frames=batch, height=height, width=width, noise=0.002)
+    gt = sc["depths"]
+    gt = torch.where(gt > 0, gt, torch.roll(gt, 1, -1)).clamp_min(0.1)[:, None]      # undo the scan's zeroed pixels
+    K4 = torch.eye(4).repeat(batch, 1, 1)
+    K4[:, :3, :3] = sc["K"]
+    noise = torch.nn.functional.avg_pool2d(torch.randn(batch, 1, height + 4, width + 4, generator=g), 5, 1)
+    pred = gt * torch.exp(pred_noise * noise * 2.0)
+    if holes:
+        v, u = torch.meshgrid(torch.arange(height), torch.arange(width), indexing="ij")
+        for b in range(batch):
+            cy, cx = torch.randint(0, height, (1,), generator=g).item(), torch.randint(0, width, (1,), generator=g).item()
+            r = max(1.0, min(height, width) / 6)
+            gt[b, 0][(v - cy) ** 2 + (u - cx) ** 2 <= r * r] = float("nan")
+            iso = torch.randint(0, height * width, (3,), generator=g)
+            gt[b, 0].view(-1)[iso] = float("nan")
+            zy, zx = torch.randint(0, height, (1,), generator=g).item(), torch.randint(0, width, (1,), generator=g).item()
+            gt[b, 0, zy:zy + max(1, height // 8), zx:zx + max(1, width // 8)] = 0.0
+    return dict(depth_gt_b1hw=gt, depth_pred_b1hw=pred, invK_b44=torch.inverse(K4))
