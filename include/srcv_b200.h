@@ -511,6 +511,52 @@ int32_t srcv_normals_loss_backward_f32(const float* normals_gt, const float* nor
                                        int32_t W, const float* grad_loss, float* grad_pred, float* grad_gt,
                                        const void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- multi-scale gradient loss (training loss, Equation 3) ------------------------------ *
+ * Replaces MSGradientLoss.forward of the reference (losses.py:11-37; depth_model.py:466, :487).
+ * DESIGN §4.14.  Level 0 is the input; level l is blur_pool2d of level l-1: the [1,2,1] x [1,2,1] / 16
+ * kernel at stride 2 with zero padding 1, size ceil(h / 2).  Per level, Gx and Gy are the Sobel
+ * gradients / 8 with replicate padding of both tensors; a gradient component is in the mask when all
+ * nine clamped window values of the ground truth at that level are finite; the level's term is the
+ * mean of |G(pred) - G(gt)| over the masked components (fp32 terms, fp64 sum, exact count), and the
+ * loss is the sum over the levels.  A level without a masked component makes the loss NaN and passes
+ * no gradient.  All pointers DEVICE memory, dense fp32:
+ *   depth_gt, depth_pred (B,1,H,W)     loss (1 float) out
+ * backward: grad_pred (B,1,H,W) out from grad_loss (1 float): per level the Sobel adjoint of
+ *   sign(delta) mask grad_loss / count, summed down the pyramid through the blur-pool adjoints.
+ *   `workspace` must be the one the forward call on the same inputs filled.
+ * Workspace layout (srcv_msgrad_workspace_bytes):
+ *   [ counts: 4 x int64 = masked components per level, 0 past num_scales; padded to 256 bytes
+ *   | partial sums (double) then partial counts (int64), one per CTA of the loss launch; padded to 256
+ *   | ground-truth pyramid: levels 1..num_scales-1, each (B,h_l,w_l) fp32 | prediction pyramid
+ *   | gradient pyramid (scratch of the backward) ]
+ * Limits (SRCV_ERR_SHAPE): num_scales in [1, 4]; H, W >= 1; 1 <= B <= 65535; B H W < 2^30.  At most three
+ * forward launches (pyramids, per-CTA partials, a fixed-order finalize) and num_scales backward
+ * launches; gather form, no atomics, no host synchronisation: bit-identical on every run.          */
+size_t srcv_msgrad_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t num_scales);
+int32_t srcv_msgrad_forward_f32(const float* depth_gt, const float* depth_pred, int32_t B, int32_t H, int32_t W,
+                                int32_t num_scales, float* loss, void* workspace, size_t workspace_bytes,
+                                void* stream);
+int32_t srcv_msgrad_backward_f32(const float* depth_gt, const float* depth_pred, int32_t B, int32_t H, int32_t W,
+                                 int32_t num_scales, const float* grad_loss, float* grad_pred, void* workspace,
+                                 size_t workspace_bytes, void* stream);
+
+/* ---- scale-invariant loss --------------------------------------------------------------- *
+ * Replaces ScaleInvariantLoss.forward of the reference (losses.py:39-54; depth_model.py:468):
+ *   loss = sqrt(mean(d^2) - si_lambda mean(d)^2),  d = log_depth_gt - log_depth_pred (n fp32 elements
+ * each, DEVICE), d in fp32, the sums and the formula in fp64.  A negative radicand or n == 0 gives NaN
+ * (with n == 0 the two inputs may be NULL).
+ * backward: grad_gt = grad_loss[0] (d - si_lambda mean(d)) / (n loss), grad_pred = -grad_gt (either may
+ *   be NULL).  `workspace` must be the one the forward call on the same inputs filled:
+ *   [ mean(d): double, loss: double, n: int64; padded to 256 bytes | partial sums of d, then of d^2 ]
+ * Limits: 0 <= n < 2^31.  Two forward launches, one backward launch (none when n == 0); bit-identical
+ * on every run.                                                                                    */
+size_t srcv_si_loss_workspace_bytes(int64_t n);
+int32_t srcv_si_loss_forward_f32(const float* log_depth_gt, const float* log_depth_pred, int64_t n, double si_lambda,
+                                 float* loss, void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_si_loss_backward_f32(const float* log_depth_gt, const float* log_depth_pred, int64_t n,
+                                  double si_lambda, const float* grad_loss, float* grad_gt, float* grad_pred,
+                                  const void* workspace, size_t workspace_bytes, void* stream);
+
 /* ---- tuning / introspection ------------------------------------------- *
  * Selects the kernel variant used by the two forward calls on this thread's
  * next invocations (process-global).  0 = automatic choice.  Used by the tests

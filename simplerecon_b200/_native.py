@@ -157,6 +157,14 @@ SYMBOLS = {
                                                   _fp]),
     "srcv_normals_loss_backward_f32": (C.c_int32, [_fp, _fp, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp, _fp,
                                                    C.c_size_t, _fp]),
+    "srcv_msgrad_workspace_bytes": (C.c_size_t, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
+    "srcv_msgrad_forward_f32": (C.c_int32, [_fp, _fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp,
+                                            C.c_size_t, _fp]),
+    "srcv_msgrad_backward_f32": (C.c_int32, [_fp, _fp, C.c_int32, C.c_int32, C.c_int32, C.c_int32, _fp, _fp, _fp,
+                                             C.c_size_t, _fp]),
+    "srcv_si_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "srcv_si_loss_forward_f32": (C.c_int32, [_fp, _fp, C.c_int64, C.c_double, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_si_loss_backward_f32": (C.c_int32, [_fp, _fp, C.c_int64, C.c_double, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_set_variant": (C.c_int32, [C.c_int32]),
     "srcv_last_variant": (C.c_char_p, []),
     "srcv_launch_count": (C.c_uint64, []),

@@ -736,6 +736,82 @@ int32_t srcv_normals_loss_backward_f32(const float* gt, const float* pred, int32
   return SRCV_OK;
 }
 
+static bool msgrad_dims_ok(int32_t B, int32_t H, int32_t W, int32_t num_scales) {
+  return B >= 1 && B <= 65535 && H >= 1 && W >= 1 && num_scales >= 1 && num_scales <= kMsGradMaxScales &&
+         (long long)B * H * W < (1ll << 30);
+}
+
+static int32_t check_msgrad(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W, int32_t num_scales,
+                            void* workspace, size_t workspace_bytes) {
+  if (!gt || !pred) return fail(SRCV_ERR_NULL, "depth_gt / depth_pred is NULL");
+  if (!msgrad_dims_ok(B, H, W, num_scales))
+    return fail(SRCV_ERR_SHAPE, "bad gradient-loss shape B=%d H=%d W=%d num_scales=%d (num_scales in [1, %d], "
+                "B <= 65535, B H W < 2^30)", B, H, W, num_scales, kMsGradMaxScales);
+  return check_workspace(workspace, workspace_bytes, msgrad_workspace_bytes(B, H, W, num_scales));
+}
+
+size_t srcv_msgrad_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t num_scales) {
+  if (!msgrad_dims_ok(B, H, W, num_scales)) return 0;
+  return msgrad_workspace_bytes(B, H, W, num_scales);
+}
+
+int32_t srcv_msgrad_forward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W, int32_t num_scales,
+                                float* loss, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!loss) return fail(SRCV_ERR_NULL, "loss is NULL");
+  if (int32_t e = check_msgrad(gt, pred, B, H, W, num_scales, workspace, workspace_bytes)) return e;
+  g_last_variant.store("msgrad_forward_f32");
+  cudaError_t err = launch_msgrad_forward(gt, pred, B, H, W, num_scales, loss, workspace,
+                                          static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "msgrad_forward");
+  return SRCV_OK;
+}
+
+int32_t srcv_msgrad_backward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W,
+                                 int32_t num_scales, const float* grad_loss, float* grad_pred, void* workspace,
+                                 size_t workspace_bytes, void* stream_) {
+  if (!grad_loss || !grad_pred) return fail(SRCV_ERR_NULL, "grad_loss / grad_pred is NULL");
+  if (int32_t e = check_msgrad(gt, pred, B, H, W, num_scales, workspace, workspace_bytes)) return e;
+  g_last_variant.store("msgrad_backward_f32");
+  cudaError_t err = launch_msgrad_backward(gt, pred, B, H, W, num_scales, grad_loss, grad_pred, workspace,
+                                           static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "msgrad_backward");
+  return SRCV_OK;
+}
+
+static int32_t check_si_loss(const float* gt, const float* pred, int64_t n, const void* workspace,
+                             size_t workspace_bytes) {
+  if (n < 0 || n >= (1ll << 31)) return fail(SRCV_ERR_SHAPE, "bad scale-invariant loss size n=%lld (0 <= n < 2^31)", (long long)n);
+  if (n > 0 && (!gt || !pred)) return fail(SRCV_ERR_NULL, "log_depth_gt / log_depth_pred is NULL");
+  return check_workspace(const_cast<void*>(workspace), workspace_bytes, si_loss_workspace_bytes(n));
+}
+
+size_t srcv_si_loss_workspace_bytes(int64_t n) {
+  if (n < 0 || n >= (1ll << 31)) return 0;
+  return si_loss_workspace_bytes(n);
+}
+
+int32_t srcv_si_loss_forward_f32(const float* gt, const float* pred, int64_t n, double si_lambda, float* loss,
+                                 void* workspace, size_t workspace_bytes, void* stream_) {
+  if (!loss) return fail(SRCV_ERR_NULL, "loss is NULL");
+  if (int32_t e = check_si_loss(gt, pred, n, workspace, workspace_bytes)) return e;
+  g_last_variant.store("si_loss_forward_f32");
+  cudaError_t err = launch_si_loss_forward(gt, pred, n, si_lambda, loss, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "si_loss_forward");
+  return SRCV_OK;
+}
+
+int32_t srcv_si_loss_backward_f32(const float* gt, const float* pred, int64_t n, double si_lambda,
+                                  const float* grad_loss, float* grad_gt, float* grad_pred, const void* workspace,
+                                  size_t workspace_bytes, void* stream_) {
+  if (!grad_loss) return fail(SRCV_ERR_NULL, "grad_loss is NULL");
+  if (int32_t e = check_si_loss(gt, pred, n, workspace, workspace_bytes)) return e;
+  g_last_variant.store("si_loss_backward_f32");
+  cudaError_t err = launch_si_loss_backward(gt, pred, n, si_lambda, grad_loss, grad_gt, grad_pred, workspace,
+                                            static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "si_loss_backward");
+  return SRCV_OK;
+}
+
 int32_t srcv_tc_selftest_f32(const float* A, const float* Wm, int32_t Kp, float* D, void* scratch,
                              void* stream) {
   if (!A || !Wm || !D || !scratch) return fail(SRCV_ERR_NULL, "selftest pointer is NULL");

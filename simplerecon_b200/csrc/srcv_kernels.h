@@ -148,6 +148,20 @@ cudaError_t launch_normals_loss_backward(const float* gt, const float* pred, int
                                          const float* grad_loss, float* grad_pred, float* grad_gt,
                                          const void* workspace, cudaStream_t stream);
 
+// multi-scale gradient loss and scale-invariant loss (csrc/srcv_gradloss.cuh, compiled in the srcv_mvloss.cu unit)
+constexpr int kMsGradMaxScales = 4;                   // pyramid levels, the input included
+size_t msgrad_workspace_bytes(int B, int H, int W, int num_scales);
+cudaError_t launch_msgrad_forward(const float* gt, const float* pred, int B, int H, int W, int num_scales, float* loss,
+                                  void* workspace, cudaStream_t stream);
+cudaError_t launch_msgrad_backward(const float* gt, const float* pred, int B, int H, int W, int num_scales,
+                                   const float* grad_loss, float* grad_pred, void* workspace, cudaStream_t stream);
+size_t si_loss_workspace_bytes(long long n);
+cudaError_t launch_si_loss_forward(const float* gt, const float* pred, long long n, double lambda, float* loss,
+                                   void* workspace, cudaStream_t stream);
+cudaError_t launch_si_loss_backward(const float* gt, const float* pred, long long n, double lambda,
+                                    const float* grad_loss, float* grad_gt, float* grad_pred, const void* workspace,
+                                    cudaStream_t stream);
+
 // argmax over planes -> plane depth (used by variants that do not fuse it)
 cudaError_t launch_argmax(const srcv_shape& s, const float* cost, const float* planes,
                           bool per_pixel, float* lowest, cudaStream_t stream);

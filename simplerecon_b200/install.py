@@ -19,6 +19,10 @@ the saved originals, so CPU callers of that utility module keep working.
 ``install(normals=True)`` swaps ``utils.geometry_utils.NormalGenerator`` and ``losses.NormalsLoss`` (the
 normals term of the training loss, depth_model.py:143, :156, :475) for the kernel-backed mirrors, and the
 names ``experiment_modules.depth_model`` binds at import (:7, :15) if it was already imported.
+``install(depth_losses=True)`` swaps ``losses.MSGradientLoss`` and ``losses.ScaleInvariantLoss`` (the gradient
+term of the training loss and the logged scale-invariant term, depth_model.py:466-468, :487) for the
+kernel-backed mirrors, and the names ``experiment_modules.depth_model`` binds at import (:7) if it was already
+imported.
 ``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
@@ -33,12 +37,12 @@ _saved: dict = {}
 
 
 def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False,
-            metrics: bool = False, normals: bool = False) -> list[str]:
+            metrics: bool = False, normals: bool = False, depth_losses: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
     with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``,
     with ``metrics=True`` also as ``utils.metrics_utils``, with ``normals=True`` also as ``losses`` and
-    ``utils.geometry_utils``."""
+    ``utils.geometry_utils``, with ``depth_losses=True`` also as ``losses``."""
     if fuse_color and not fusion:
         raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
     from . import cost_volume as ours
@@ -96,6 +100,15 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
                     setattr(mod, n, getattr(ours_normals, n))
                     if mod.__name__ not in patched:
                         patched.append(mod.__name__)
+    if depth_losses:
+        from . import losses as ours_losses
+        for mod in [importlib.import_module("losses")] + ([dm] if dm is not None else []):
+            for n in ("MSGradientLoss", "ScaleInvariantLoss"):
+                if hasattr(mod, n):
+                    _saved.setdefault((mod.__name__, n), getattr(mod, n))
+                    setattr(mod, n, getattr(ours_losses, n))
+            if mod.__name__ not in patched:
+                patched.append(mod.__name__)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched

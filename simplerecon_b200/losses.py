@@ -1,4 +1,6 @@
-"""Multi-view depth regression loss, backed by the sm_90a kernel.
+"""The training losses of the reference's ``losses.py``, backed by the sm_90a kernels: ``MVDepthLoss`` (below),
+``MSGradientLoss`` and ``ScaleInvariantLoss`` (csrc/srcv_gradloss.cuh, DESIGN §4.14; at the end of this module).
+``NormalsLoss`` lives in ``normals.py`` with the generator it consumes.
 
 Mirrors ``MVDepthLoss`` of the reference's ``losses.py`` (:79-208) — constructor ``(height, width)``,
 ``forward`` with the reference's keyword names (``experiment_modules/depth_model.py:477-485`` calls it
@@ -25,7 +27,7 @@ from . import _native
 def _require_cuda(t: torch.Tensor) -> None:
     """The device gate (tests/ patch exactly this to drive the host-emulated library)."""
     if t.device.type != "cuda":
-        raise RuntimeError("simplerecon_b200 MVDepthLoss runs on CUDA (sm_90a) only; there is no CPU fallback")
+        raise RuntimeError("simplerecon_b200 losses run on CUDA (sm_90a) only; there is no CPU fallback")
 
 
 def _lib():
@@ -135,3 +137,126 @@ class MVDepthLoss(nn.Module):
         _require_cuda(depth_pred_b1hw)
         return _MvLossFunction.apply(depth_pred_b1hw, cur_depth_b1hw, src_depth_bk1hw, cur_invK_b44, src_K_bk44,
                                      cur_world_T_cam_b44, src_cam_T_world_bk44)
+
+
+def _msgrad_forward(depth_gt: torch.Tensor, depth_pred: torch.Tensor, num_scales: int):
+    """(loss, workspace) of dense fp32 inputs.  The workspace starts with the four int64 counts of masked
+    gradient components per level and keeps both pyramids for the backward (include/srcv_b200.h)."""
+    B, _, H, W = depth_gt.shape
+    dev = depth_gt.device
+    n = _lib().srcv_msgrad_workspace_bytes(B, H, W, num_scales)
+    if n == 0:
+        raise ValueError(f"unsupported depth shape {tuple(depth_gt.shape)} (B <= 65535, B H W < 2^30)")
+    ws = torch.empty(n, device=dev, dtype=torch.uint8)
+    loss = torch.empty((), device=dev, dtype=torch.float32)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_msgrad_forward_f32(
+            C.c_void_p(depth_gt.data_ptr()), C.c_void_p(depth_pred.data_ptr()), B, H, W, num_scales,
+            C.c_void_p(loss.data_ptr()), C.c_void_p(ws.data_ptr()), n, _stream(dev)))
+    return loss, ws
+
+
+class _MsGradFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, depth_gt, depth_pred, num_scales):
+        gt, pred = _f32c(depth_gt), _f32c(depth_pred)
+        loss, ws = _msgrad_forward(gt, pred, num_scales)
+        ctx.save_for_backward(gt, pred, ws)     # the workspace keeps the pyramids and the per-level counts
+        ctx.num_scales = num_scales
+        ctx.pred_dtype = depth_pred.dtype
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        gt, pred, ws = ctx.saved_tensors
+        B, _, H, W = gt.shape
+        dev = gt.device
+        g = _f32c(grad_loss).reshape(1)
+        out = torch.empty_like(pred)
+        with torch.cuda.device(dev):
+            _native.check(_lib().srcv_msgrad_backward_f32(
+                C.c_void_p(gt.data_ptr()), C.c_void_p(pred.data_ptr()), B, H, W, ctx.num_scales,
+                C.c_void_p(g.data_ptr()), C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(),
+                _stream(dev)))
+        return None, out.to(ctx.pred_dtype), None
+
+
+class MSGradientLoss(nn.Module):
+    """reference losses.py:11-37 (Equation 3 of the paper): the sum over ``num_scales`` blur-pool pyramid levels
+    of the mean absolute difference of the Sobel gradients, over the gradient components whose ground-truth
+    window is finite.  Differentiable w.r.t. ``depth_pred`` only: ``depth_gt`` is data, as in ``MVDepthLoss``.
+    Three launches forward, ``num_scales`` backward, no host synchronisation.  Half / bfloat16 inputs are
+    computed in fp32; the loss is fp32 and the gradient comes back in the prediction's dtype."""
+
+    MAX_SCALES = 4
+
+    def __init__(self, num_scales: int = 4):
+        super().__init__()
+        if not 1 <= num_scales <= self.MAX_SCALES:
+            raise ValueError(f"num_scales must be in [1, {self.MAX_SCALES}] (the pyramid kernel's depth), "
+                             f"got {num_scales}")
+        self.num_scales = num_scales
+
+    def forward(self, depth_gt: torch.Tensor, depth_pred: torch.Tensor) -> torch.Tensor:
+        _require_cuda(depth_pred)
+        if depth_gt.dim() != 4 or depth_gt.shape[1] != 1 or depth_gt.shape != depth_pred.shape:
+            raise ValueError(f"depths must both be (B, 1, H, W), got {tuple(depth_gt.shape)} and "
+                             f"{tuple(depth_pred.shape)}")
+        if depth_gt.device != depth_pred.device:
+            raise ValueError(f"depths on {depth_gt.device} and {depth_pred.device}")
+        return _MsGradFunction.apply(depth_gt, depth_pred, self.num_scales)
+
+
+class _SiLossFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, log_depth_gt, log_depth_pred, si_lambda):
+        gt, pred = _f32c(log_depth_gt), _f32c(log_depth_pred)
+        dev, count = gt.device, gt.numel()
+        n = _lib().srcv_si_loss_workspace_bytes(count)
+        if n == 0:
+            raise ValueError(f"unsupported input size {count} (at most 2^31 - 1 elements)")
+        ws = torch.empty(n, device=dev, dtype=torch.uint8)
+        loss = torch.empty((), device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            _native.check(_lib().srcv_si_loss_forward_f32(
+                C.c_void_p(gt.data_ptr()), C.c_void_p(pred.data_ptr()), count, si_lambda,
+                C.c_void_p(loss.data_ptr()), C.c_void_p(ws.data_ptr()), n, _stream(dev)))
+        ctx.save_for_backward(gt, pred, ws)     # the workspace keeps mean(d) and the loss
+        ctx.si_lambda = si_lambda
+        ctx.dtypes = (log_depth_gt.dtype, log_depth_pred.dtype)
+        return loss
+
+    @staticmethod
+    def backward(ctx, grad_loss):
+        gt, pred, ws = ctx.saved_tensors
+        dev = gt.device
+        g = _f32c(grad_loss).reshape(1)
+        g_gt = torch.empty_like(gt) if ctx.needs_input_grad[0] else None
+        g_pred = torch.empty_like(pred) if ctx.needs_input_grad[1] else None
+        with torch.cuda.device(dev):
+            _native.check(_lib().srcv_si_loss_backward_f32(
+                C.c_void_p(gt.data_ptr()), C.c_void_p(pred.data_ptr()), gt.numel(), ctx.si_lambda,
+                C.c_void_p(g.data_ptr()), C.c_void_p(g_gt.data_ptr() if g_gt is not None else 0),
+                C.c_void_p(g_pred.data_ptr() if g_pred is not None else 0), C.c_void_p(ws.data_ptr()), ws.numel(),
+                _stream(dev)))
+        return (g_gt.to(ctx.dtypes[0]) if g_gt is not None else None,
+                g_pred.to(ctx.dtypes[1]) if g_pred is not None else None, None)
+
+
+class ScaleInvariantLoss(nn.Module):
+    """reference losses.py:39-54: ``sqrt(mean(d^2) - si_lambda mean(d)^2)`` with ``d = log_depth_gt -
+    log_depth_pred``, any equal shape (the caller passes the 1-D ``x[mask_b]``, depth_model.py:468).  ``d`` is
+    fp32, the sums and the formula fp64; NaN for a negative radicand or an empty input, as ``torch.sqrt`` and
+    ``mean`` give.  Differentiable in both inputs.  Two launches forward, one backward."""
+
+    def __init__(self, si_lambda: float = 0.85):
+        super().__init__()
+        self.si_lambda = si_lambda
+
+    def forward(self, log_depth_gt: torch.Tensor, log_depth_pred: torch.Tensor) -> torch.Tensor:
+        _require_cuda(log_depth_pred)
+        if log_depth_gt.shape != log_depth_pred.shape:
+            raise ValueError(f"shapes differ: {tuple(log_depth_gt.shape)} and {tuple(log_depth_pred.shape)}")
+        if log_depth_gt.device != log_depth_pred.device:
+            raise ValueError(f"inputs on {log_depth_gt.device} and {log_depth_pred.device}")
+        return _SiLossFunction.apply(log_depth_gt, log_depth_pred, float(self.si_lambda))
