@@ -557,6 +557,49 @@ int32_t srcv_si_loss_backward_f32(const float* log_depth_gt, const float* log_de
                                   double si_lambda, const float* grad_loss, float* grad_gt, float* grad_pred,
                                   const void* workspace, size_t workspace_bytes, void* stream);
 
+/* ---- regression terms of the training loss (Equation 2 and the logged terms) ------------ *
+ * Replaces lines 447-474 of DepthModel.compute_losses of the reference (experiment_modules/depth_model.py).
+ * DESIGN §4.15.  Over the whole batch, with lg = log(gt) in fp32 and n = the number of pixels whose mask byte is
+ * nonzero:
+ *   ms_loss      = sum over the present scales i of mean_mask |lg - lp_i(nearest)| / 2^i, lp_i sampled at
+ *                  PyTorch's nearest source index min(floor(dst * in/out), in - 1) (fp32 scale)
+ *   abs_loss     = mean_mask |gt - depth_pred|            log_l1_loss = mean_mask |lg - lp_0|
+ *   si_loss      = sqrt(mean(d^2) - si_lambda mean(d)^2), d = lg - lp_0 over the mask
+ *   inv_abs_loss = mean |1/gt - 1/depth_pred| over the mask and depth_pred > 0.1f (its own count m)
+ * fp32 terms, fp64 sums, exact counts; an empty mask (n = 0, or m = 0 for inv_abs_loss) gives NaN.  Values
+ * outside the mask are never read as terms, so NaN ground truth there is ignored.  All pointers DEVICE memory,
+ * dense:
+ *   gt, depth_pred (B,1,H,W) fp32   mask (B,1,H,W) uint8   log_pred[i] (B,1,h[i],w[i]) fp32 or NULL (absent)
+ *   losses (5 floats) out, in the order ms_loss, abs_loss, si_loss, inv_abs_loss, log_l1_loss
+ * backward: grad_losses[5] point to the upstream gradient of each loss in the same order (NULL, or a zero, adds
+ *   nothing: an output autograd did not reach); grad_log_pred[i] (B,1,h[i],w[i]) and grad_depth_pred (B,1,H,W)
+ *   out, each may be NULL (not wanted).  At scale i >= 1 the gradient is sign(lp_i - lg) mask g_ms / (n 2^i)
+ *   summed over the pixel's nearest-resampling preimage (0 for an empty preimage); sign(0) = sign(NaN) = 0.
+ *   `workspace` must be the one the forward call on the same inputs filled.
+ * Workspace layout (srcv_regloss_workspace_bytes):
+ *   [ n, m: int64; mean(d), si_loss: double; padded to 256 bytes
+ *   | partial sums: 6 series (ms, abs, log_l1, d, d^2, inv_abs) of one double per forward CTA
+ *   | partial counts: 2 series (n, m) of one int64 per forward CTA; padded to 256 ]
+ * Limits (SRCV_ERR_SHAPE): 1 <= B <= 65535; H, W >= 1; B H W < 2^30; log_pred[0] required (SRCV_ERR_NULL)
+ *   with h[0] = H, w[0] = W; every present scale h[i], w[i] >= 1 with B h[i] w[i] < 2^30.  Two forward
+ *   launches (per-CTA partials, a fixed-order finalize), one backward launch; gather form, no atomics, no host
+ *   synchronisation: bit-identical on every run.                                                      */
+typedef struct srcv_regloss_args {
+  const float* gt;
+  const uint8_t* mask;
+  const float* depth_pred;
+  const float* log_pred[4];
+  int32_t h[4], w[4];
+  int32_t B, H, W;
+  double si_lambda;
+} srcv_regloss_args;
+size_t srcv_regloss_workspace_bytes(const srcv_regloss_args* args);
+int32_t srcv_regloss_forward_f32(const srcv_regloss_args* args, float* losses, void* workspace, size_t workspace_bytes,
+                                 void* stream);
+int32_t srcv_regloss_backward_f32(const srcv_regloss_args* args, const float* const grad_losses[5],
+                                  float* const grad_log_pred[4], float* grad_depth_pred, const void* workspace,
+                                  size_t workspace_bytes, void* stream);
+
 /* ---- tuning / introspection ------------------------------------------- *
  * Selects the kernel variant used by the two forward calls on this thread's
  * next invocations (process-global).  0 = automatic choice.  Used by the tests

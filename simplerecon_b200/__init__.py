@@ -23,5 +23,6 @@ from .tsdf import TSDF, TSDFFuser  # noqa: E402,F401  (reference tools/tsdf.py)
 from .fusers import ColorFuser  # noqa: E402,F401  (OurFuser with colour, DESIGN §4.11)
 from . import point_cloud_fusion  # noqa: E402,F401  (reference tools/torch_point_cloud_fusion.py)
 from .losses import MSGradientLoss, MVDepthLoss, ScaleInvariantLoss  # noqa: E402,F401  (reference losses.py:11-54, :79-208)
+from .losses import depth_regression_losses  # noqa: E402,F401  (reference experiment_modules/depth_model.py:447-474)
 from .metrics import compute_depth_metrics, compute_depth_metrics_batched, depth_metrics  # noqa: E402,F401  (reference utils/metrics_utils.py)
 from .normals import NormalGenerator, NormalsLoss  # noqa: E402,F401  (reference geometry_utils.py:92-133, losses.py:57-77)

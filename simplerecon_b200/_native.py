@@ -101,6 +101,11 @@ class NormalsArgs(C.Structure):
     _fields_ = [("depth", _fp), ("invK", _fp), ("taps", _fp)] + [(n, C.c_int32) for n in ("B", "H", "W", "k")]
 
 
+class RegLossArgs(C.Structure):
+    _fields_ = [("gt", _fp), ("mask", _fp), ("depth_pred", _fp), ("log_pred", _fp * 4), ("h", C.c_int32 * 4),
+                ("w", C.c_int32 * 4), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("si_lambda", C.c_double)]
+
+
 # every symbol include/srcv_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "srcv_abi_version": (C.c_int32, []),
@@ -165,6 +170,10 @@ SYMBOLS = {
     "srcv_si_loss_workspace_bytes": (C.c_size_t, [C.c_int64]),
     "srcv_si_loss_forward_f32": (C.c_int32, [_fp, _fp, C.c_int64, C.c_double, _fp, _fp, C.c_size_t, _fp]),
     "srcv_si_loss_backward_f32": (C.c_int32, [_fp, _fp, C.c_int64, C.c_double, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_regloss_workspace_bytes": (C.c_size_t, [C.POINTER(RegLossArgs)]),
+    "srcv_regloss_forward_f32": (C.c_int32, [C.POINTER(RegLossArgs), _fp, _fp, C.c_size_t, _fp]),
+    "srcv_regloss_backward_f32": (C.c_int32, [C.POINTER(RegLossArgs), C.POINTER(_fp), C.POINTER(_fp), _fp, _fp,
+                                              C.c_size_t, _fp]),
     "srcv_set_variant": (C.c_int32, [C.c_int32]),
     "srcv_last_variant": (C.c_char_p, []),
     "srcv_launch_count": (C.c_uint64, []),

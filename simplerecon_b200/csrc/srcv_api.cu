@@ -812,6 +812,53 @@ int32_t srcv_si_loss_backward_f32(const float* gt, const float* pred, int64_t n,
   return SRCV_OK;
 }
 
+static bool regloss_dims_ok(const srcv_regloss_args* a) {
+  if (a->B < 1 || a->B > 65535 || a->H < 1 || a->W < 1 || (long long)a->B * a->H * a->W >= (1ll << 30)) return false;
+  if (a->h[0] != a->H || a->w[0] != a->W) return false;
+  for (int i = 1; i < kRegLossMaxScales; ++i)
+    if (a->log_pred[i] && (a->h[i] < 1 || a->w[i] < 1 || (long long)a->B * a->h[i] * a->w[i] >= (1ll << 30)))
+      return false;
+  return true;
+}
+
+static int32_t check_regloss(const srcv_regloss_args* a, const void* workspace, size_t workspace_bytes) {
+  if (!a) return fail(SRCV_ERR_NULL, "regression-loss arguments are NULL");
+  if (!a->gt || !a->mask || !a->depth_pred) return fail(SRCV_ERR_NULL, "gt / mask / depth_pred is NULL");
+  if (!a->log_pred[0]) return fail(SRCV_ERR_NULL, "log_pred[0] is NULL (scale 0 is required)");
+  if (!regloss_dims_ok(a))
+    return fail(SRCV_ERR_SHAPE, "bad regression-loss shape B=%d H=%d W=%d, scales %dx%d %dx%d %dx%d %dx%d (B <= 65535, "
+                "scale 0 = H x W, present scales >= 1x1, B H W and B h w < 2^30)", a->B, a->H, a->W, a->h[0], a->w[0],
+                a->h[1], a->w[1], a->h[2], a->w[2], a->h[3], a->w[3]);
+  return check_workspace(const_cast<void*>(workspace), workspace_bytes, regloss_workspace_bytes(*a));
+}
+
+size_t srcv_regloss_workspace_bytes(const srcv_regloss_args* a) {
+  if (!a || !a->log_pred[0] || !regloss_dims_ok(a)) return 0;
+  return regloss_workspace_bytes(*a);
+}
+
+int32_t srcv_regloss_forward_f32(const srcv_regloss_args* a, float* losses, void* workspace, size_t workspace_bytes,
+                                 void* stream_) {
+  if (!losses) return fail(SRCV_ERR_NULL, "losses is NULL");
+  if (int32_t e = check_regloss(a, workspace, workspace_bytes)) return e;
+  g_last_variant.store("regloss_forward_f32");
+  cudaError_t err = launch_regloss_forward(*a, losses, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "regloss_forward");
+  return SRCV_OK;
+}
+
+int32_t srcv_regloss_backward_f32(const srcv_regloss_args* a, const float* const grad_losses[5],
+                                  float* const grad_log_pred[4], float* grad_depth_pred, const void* workspace,
+                                  size_t workspace_bytes, void* stream_) {
+  if (!grad_losses || !grad_log_pred) return fail(SRCV_ERR_NULL, "grad_losses / grad_log_pred array is NULL");
+  if (int32_t e = check_regloss(a, workspace, workspace_bytes)) return e;
+  g_last_variant.store("regloss_backward_f32");
+  cudaError_t err = launch_regloss_backward(*a, grad_losses, grad_log_pred, grad_depth_pred, workspace,
+                                            static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "regloss_backward");
+  return SRCV_OK;
+}
+
 int32_t srcv_tc_selftest_f32(const float* A, const float* Wm, int32_t Kp, float* D, void* scratch,
                              void* stream) {
   if (!A || !Wm || !D || !scratch) return fail(SRCV_ERR_NULL, "selftest pointer is NULL");

@@ -162,6 +162,14 @@ cudaError_t launch_si_loss_backward(const float* gt, const float* pred, long lon
                                     const float* grad_loss, float* grad_gt, float* grad_pred, const void* workspace,
                                     cudaStream_t stream);
 
+// the regression terms of the training loss (csrc/srcv_regloss.cuh, compiled in the srcv_mvloss.cu unit)
+constexpr int kRegLossMaxScales = 4;                  // decoder scales s0..s3
+size_t regloss_workspace_bytes(const srcv_regloss_args& a);
+cudaError_t launch_regloss_forward(const srcv_regloss_args& a, float* losses, void* workspace, cudaStream_t stream);
+cudaError_t launch_regloss_backward(const srcv_regloss_args& a, const float* const grad_losses[5],
+                                    float* const grad_log_pred[kRegLossMaxScales], float* grad_depth_pred,
+                                    const void* workspace, cudaStream_t stream);
+
 // argmax over planes -> plane depth (used by variants that do not fuse it)
 cudaError_t launch_argmax(const srcv_shape& s, const float* cost, const float* planes,
                           bool per_pixel, float* lowest, cudaStream_t stream);

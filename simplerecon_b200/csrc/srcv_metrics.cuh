@@ -18,6 +18,13 @@
 
 namespace srcv {
 
+// PyTorch's nearest source index (F.interpolate mode="nearest", output size given): min(floor(dst * scale), in - 1)
+// with the fp32 scale = in / out.  A same-size input maps every index to itself.  Shared with the regression-loss
+// kernels (srcv_regloss.cuh), whose backward inverts this map by searching it.
+__device__ __forceinline__ int nearest_src_index(int dst, float scale, int in) {
+  return min((int)floorf(__fmul_rn((float)dst, scale)), in - 1);
+}
+
 namespace metrics_detail {
 namespace {
 
@@ -59,8 +66,7 @@ __device__ __forceinline__ float linear_src(float scale, int dst) {
 __device__ __forceinline__ float sample_pred(const srcv_metrics_args& a, const float* __restrict__ pred, int x, int y,
                                              int p, float sy, float sx) {
   if (a.resample == SRCV_RESAMPLE_NEAREST) {       // min(floor(dst * in/out), in - 1)
-    const int iy = min((int)floorf(__fmul_rn((float)y, sy)), a.Hp - 1);
-    const int ix = min((int)floorf(__fmul_rn((float)x, sx)), a.Wp - 1);
+    const int iy = nearest_src_index(y, sy, a.Hp), ix = nearest_src_index(x, sx, a.Wp);
     return __ldg(pred + iy * a.Wp + ix);
   }
   if (a.resample == SRCV_RESAMPLE_BILINEAR) {

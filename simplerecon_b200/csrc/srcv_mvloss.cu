@@ -226,3 +226,4 @@ cudaError_t launch_mvloss_backward(const srcv_mvloss_args& a, const float* grad_
 #include "srcv_metrics.cuh"   // depth metrics (DESIGN §4.12), compiled in this unit
 #include "srcv_normals.cuh"   // surface normals and the normals loss (DESIGN §4.13), compiled in this unit
 #include "srcv_gradloss.cuh"  // multi-scale gradient and scale-invariant losses (DESIGN §4.14), compiled in this unit
+#include "srcv_regloss.cuh"   // the regression terms of the training loss (DESIGN §4.15), compiled in this unit

@@ -23,6 +23,11 @@ names ``experiment_modules.depth_model`` binds at import (:7, :15) if it was alr
 term of the training loss and the logged scale-invariant term, depth_model.py:466-468, :487) for the
 kernel-backed mirrors, and the names ``experiment_modules.depth_model`` binds at import (:7) if it was already
 imported.
+``install(regression_losses=True)`` imports ``experiment_modules.depth_model`` and replaces
+``DepthModel.compute_losses`` (:409-500) with ``losses.compute_losses``: the multi-scale log-L1 loss and the logged
+regression terms from one fused call, the other terms from the model's own loss modules.  Models whose multi-scale
+loss is not the mean ``nn.L1Loss``, and CPU ground truth, go to the saved original.  With this flag the other flags
+also patch ``experiment_modules.depth_model``, since it is imported first.
 ``uninstall()`` restores everything.  See INTEGRATION.md.
 """
 from __future__ import annotations
@@ -37,18 +42,22 @@ _saved: dict = {}
 
 
 def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False,
-            metrics: bool = False, normals: bool = False, depth_losses: bool = False) -> list[str]:
+            metrics: bool = False, normals: bool = False, depth_losses: bool = False,
+            regression_losses: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
     with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``,
     with ``metrics=True`` also as ``utils.metrics_utils``, with ``normals=True`` also as ``losses`` and
-    ``utils.geometry_utils``, with ``depth_losses=True`` also as ``losses``."""
+    ``utils.geometry_utils``, with ``depth_losses=True`` also as ``losses``, with ``regression_losses=True``
+    also as ``experiment_modules.depth_model``."""
     if fuse_color and not fusion:
         raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
     from . import cost_volume as ours
     patched = []
     ref_cv = importlib.import_module("modules.cost_volume")
     targets = [ref_cv]
+    if regression_losses:
+        importlib.import_module("experiment_modules.depth_model")
     dm = sys.modules.get("experiment_modules.depth_model")
     if dm is not None:
         targets.append(dm)
@@ -109,6 +118,12 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
                     setattr(mod, n, getattr(ours_losses, n))
             if mod.__name__ not in patched:
                 patched.append(mod.__name__)
+    if regression_losses:
+        from .losses import compute_losses
+        _saved.setdefault((dm.__name__, "DepthModel.compute_losses"), dm.DepthModel.compute_losses)
+        dm.DepthModel.compute_losses = compute_losses
+        if dm.__name__ not in patched:
+            patched.append(dm.__name__)
     if verbose:
         print(f"simplerecon_b200: installed fused cost-volume managers into {patched}")
     return patched
@@ -142,9 +157,20 @@ def _cuda_or_original(fast, original):
     return metrics_fn
 
 
+def saved_original(mod_name: str, name: str):
+    """What ``install`` replaced under ``name`` (``Class.attr`` for a class attribute) in module ``mod_name``."""
+    try:
+        return _saved[(mod_name, name)]
+    except KeyError:
+        raise RuntimeError(f"{mod_name}.{name} has not been replaced by install(): no original to call") from None
+
+
 def uninstall() -> None:
     for (mod_name, n), cls in list(_saved.items()):
         mod = sys.modules.get(mod_name)
         if mod is not None:
-            setattr(mod, n, cls)
+            *owner, attr = n.split(".")              # "Class.attr" names a class attribute
+            for o in owner:
+                mod = getattr(mod, o)
+            setattr(mod, attr, cls)
     _saved.clear()

@@ -1,6 +1,8 @@
 """The training losses of the reference's ``losses.py``, backed by the sm_90a kernels: ``MVDepthLoss`` (below),
-``MSGradientLoss`` and ``ScaleInvariantLoss`` (csrc/srcv_gradloss.cuh, DESIGN §4.14; at the end of this module).
-``NormalsLoss`` lives in ``normals.py`` with the generator it consumes.
+``MSGradientLoss`` and ``ScaleInvariantLoss`` (csrc/srcv_gradloss.cuh, DESIGN §4.14).  ``NormalsLoss`` lives in
+``normals.py`` with the generator it consumes.  At the end of this module, the regression terms the reference
+computes inline in ``DepthModel.compute_losses`` (``depth_regression_losses``, csrc/srcv_regloss.cuh, DESIGN §4.15)
+and a drop-in ``compute_losses`` built on all of them.
 
 Mirrors ``MVDepthLoss`` of the reference's ``losses.py`` (:79-208) — constructor ``(height, width)``,
 ``forward`` with the reference's keyword names (``experiment_modules/depth_model.py:477-485`` calls it
@@ -260,3 +262,154 @@ class ScaleInvariantLoss(nn.Module):
         if log_depth_gt.device != log_depth_pred.device:
             raise ValueError(f"inputs on {log_depth_gt.device} and {log_depth_pred.device}")
         return _SiLossFunction.apply(log_depth_gt, log_depth_pred, float(self.si_lambda))
+
+
+# ---- the regression terms of compute_losses (csrc/srcv_regloss.cuh, DESIGN §4.15) ---------------------------------
+
+REGRESSION_KEYS = ("ms_loss", "abs_loss", "si_loss", "inv_abs_loss", "log_l1_loss")   # the kernel's output order
+NUM_SCALES = 4                                                                         # log_depth_pred_s0..s3
+
+
+def _regloss_call(gt, mask, depth_pred, log_preds, si_lambda):
+    """(args, workspace) of dense inputs: fp32 depths, uint8 mask, log_preds a list of four fp32 tensors or None."""
+    B, _, H, W = gt.shape
+    hs = [int(t.shape[-2]) if t is not None else 0 for t in log_preds]
+    ws_ = [int(t.shape[-1]) if t is not None else 0 for t in log_preds]
+    args = _native.RegLossArgs(
+        C.c_void_p(gt.data_ptr()), C.c_void_p(mask.data_ptr()), C.c_void_p(depth_pred.data_ptr()),
+        (C.c_void_p * 4)(*[t.data_ptr() if t is not None else None for t in log_preds]),
+        (C.c_int32 * 4)(*hs), (C.c_int32 * 4)(*ws_), B, H, W, si_lambda)
+    n = _lib().srcv_regloss_workspace_bytes(C.byref(args))
+    if n == 0:
+        raise ValueError(f"unsupported shapes: depth {tuple(gt.shape)}, scales "
+                         f"{[tuple(t.shape) if t is not None else None for t in log_preds]} "
+                         "(B <= 65535, B H W < 2^30, every scale at least 1x1)")
+    return args, torch.empty(n, device=gt.device, dtype=torch.uint8)
+
+
+class _RegLossFunction(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, depth_gt, mask_b, depth_pred, si_lambda, *log_preds):
+        gt, dp = _f32c(depth_gt), _f32c(depth_pred)
+        mask = mask_b.detach().contiguous().view(torch.uint8)
+        lps = [_f32c(t) if t is not None else None for t in log_preds]
+        args, ws = _regloss_call(gt, mask, dp, lps, si_lambda)
+        dev = gt.device
+        out = torch.empty(len(REGRESSION_KEYS), device=dev, dtype=torch.float32)
+        with torch.cuda.device(dev):
+            _native.check(_lib().srcv_regloss_forward_f32(C.byref(args), C.c_void_p(out.data_ptr()),
+                                                          C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+        ctx.set_materialize_grads(False)     # an output autograd did not reach passes NULL: it adds nothing
+        ctx.save_for_backward(gt, mask, dp, ws, *lps)   # the workspace keeps n, m, mean(d) and si
+        ctx.args = args
+        ctx.dtypes = (depth_pred.dtype, [t.dtype if t is not None else None for t in log_preds])
+        return tuple(out.unbind(0))
+
+    @staticmethod
+    def backward(ctx, *grads):
+        gt, mask, dp, ws, *lps = ctx.saved_tensors
+        dev = gt.device
+        ups = [_f32c(g) if g is not None else None for g in grads]
+        want = ctx.needs_input_grad
+        g_lp = [torch.empty_like(t) if t is not None and want[4 + i] else None for i, t in enumerate(lps)]
+        g_dp = torch.empty_like(dp) if want[2] else None
+        ptr = lambda t: t.data_ptr() if t is not None else None   # noqa: E731
+        with torch.cuda.device(dev):
+            _native.check(_lib().srcv_regloss_backward_f32(
+                C.byref(ctx.args), (C.c_void_p * 5)(*map(ptr, ups)), (C.c_void_p * 4)(*map(ptr, g_lp)),
+                C.c_void_p(ptr(g_dp)), C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+        dp_dtype, lp_dtypes = ctx.dtypes
+        return (None, None, g_dp.to(dp_dtype) if g_dp is not None else None, None,
+                *[g.to(d) if g is not None else None for g, d in zip(g_lp, lp_dtypes)])
+
+
+def depth_regression_losses(depth_gt_b1hw: torch.Tensor, mask_b_b1hw: torch.Tensor, log_depth_preds: dict,
+                            depth_pred_b1hw: torch.Tensor, si_lambda: float = 0.85) -> dict:
+    """The regression terms of the reference's ``DepthModel.compute_losses`` (experiment_modules/depth_model.py:
+    447-474) in one fused call: ``dict(ms_loss, abs_loss, si_loss, inv_abs_loss, log_l1_loss)`` of fp32 0-d tensors.
+
+    ``log_depth_preds`` maps a scale index (0..3) to ``log_depth_pred_s{i}_b1hw``; scale 0 is required and has the
+    ground truth's (B, 1, H, W) shape, the others may be absent or any size (each is nearest-resampled to the ground
+    truth, as ``F.interpolate`` does).  ``mask_b_b1hw`` is the boolean ``mask_b``.  ``ms_loss`` is the sum over the
+    present scales i of the masked mean of ``|log gt - log_depth_pred_s{i}|`` / 2^i; ``si_loss`` uses ``si_lambda``;
+    ``inv_abs_loss`` is over ``mask_b & (depth_pred > 0.1)``.  An empty mask gives NaN, as the mean of an empty
+    tensor does.  Differentiable w.r.t. every ``log_depth_pred_s{i}`` and ``depth_pred`` (separate inputs, as in the
+    reference, where ``depth_pred = exp(log_depth_pred_s0)`` is its own autograd node); the ground truth is data.
+    Two launches forward, one backward, no host synchronisation.  Half / bfloat16 inputs are computed in fp32; the
+    losses are fp32 and gradients come back in each input's dtype."""
+    _require_cuda(depth_gt_b1hw)
+    if depth_gt_b1hw.dim() != 4 or depth_gt_b1hw.shape[1] != 1:
+        raise ValueError(f"depth_gt_b1hw must be (B, 1, H, W), got {tuple(depth_gt_b1hw.shape)}")
+    shape = depth_gt_b1hw.shape
+    if set(log_depth_preds) - set(range(NUM_SCALES)):
+        raise ValueError(f"scale indices must be in 0..{NUM_SCALES - 1}, got {sorted(log_depth_preds)}")
+    if 0 not in log_depth_preds:
+        raise ValueError("log_depth_preds needs scale 0")
+    for name, t in (("mask_b_b1hw", mask_b_b1hw), ("depth_pred_b1hw", depth_pred_b1hw), ("scale 0", log_depth_preds[0])):
+        if t.shape != shape:
+            raise ValueError(f"{name} must have the ground truth's shape {tuple(shape)}, got {tuple(t.shape)}")
+    if mask_b_b1hw.dtype != torch.bool:
+        raise ValueError(f"mask_b_b1hw must be bool, got {mask_b_b1hw.dtype}")
+    lps = [log_depth_preds.get(i) for i in range(NUM_SCALES)]
+    for i, t in enumerate(lps):
+        if t is not None and (t.dim() != 4 or t.shape[:2] != shape[:2] or t.numel() == 0):
+            raise ValueError(f"scale {i} must be (B, 1, h, w) with B = {shape[0]} and h, w >= 1, got {tuple(t.shape)}")
+    tensors = [depth_gt_b1hw, mask_b_b1hw, depth_pred_b1hw, *[t for t in lps if t is not None]]
+    if any(t.device != depth_gt_b1hw.device for t in tensors):
+        raise ValueError("inputs live on different devices: " + ", ".join(str(t.device) for t in tensors))
+    outs = _RegLossFunction.apply(depth_gt_b1hw, mask_b_b1hw, depth_pred_b1hw, float(si_lambda), *lps)
+    return dict(zip(REGRESSION_KEYS, outs))
+
+
+def uses_fused_regression_losses(model, depth_gt) -> bool:
+    """Whether ``compute_losses`` runs the fused kernels for this model and ground truth: CUDA ground truth, and the
+    multi-scale loss being the model's ``abs_loss``, a mean-reduced ``nn.L1Loss`` (``loss_type == "log_l1"``,
+    depth_model.py:142, :150-151).  Anything else goes to the reference's original."""
+    abs_loss = getattr(model, "abs_loss", None)
+    return (torch.is_tensor(depth_gt) and depth_gt.is_cuda and getattr(model, "ms_loss_fn", None) is abs_loss
+            and isinstance(abs_loss, nn.L1Loss) and abs_loss.reduction == "mean")
+
+
+def compute_losses(self, cur_data, src_data, outputs):
+    """Drop-in ``DepthModel.compute_losses`` (experiment_modules/depth_model.py:409-500), assigned to the class by
+    ``install(regression_losses=True)``: the same nine losses under the same keys in the same order.  ``ms_loss``,
+    ``abs_loss``, ``si_loss``, ``inv_abs_loss`` and ``log_l1_loss`` come from one ``depth_regression_losses`` call;
+    ``grad_loss``, ``normals_loss`` and ``mv_loss`` from the model's own ``grad_loss``, ``normals_loss`` and
+    ``mv_depth_loss`` modules with the reference's arguments (kernel-backed when those were installed too).  When
+    ``uses_fused_regression_losses`` is false the call goes to the reference's saved original."""
+    depth_gt = cur_data["depth_b1hw"]
+    if not uses_fused_regression_losses(self, depth_gt):
+        from .install import saved_original
+        return saved_original("experiment_modules.depth_model", "DepthModel.compute_losses")(
+            self, cur_data, src_data, outputs)
+    log_preds = {i: outputs[f"log_depth_pred_s{i}_b1hw"] for i in range(NUM_SCALES)
+                 if f"log_depth_pred_s{i}_b1hw" in outputs}
+    if not log_preds:
+        raise Exception("Could not find a valid scale to compute si loss!")
+    depth_pred = outputs["depth_pred_s0_b1hw"]
+    log_preds[0] = outputs["log_depth_pred_s0_b1hw"]      # a KeyError without scale 0, as the reference's :444
+    terms = depth_regression_losses(depth_gt, cur_data["mask_b_b1hw"], log_preds, depth_pred,
+                                    si_lambda=float(self.si_loss.si_lambda))
+    grad_loss = self.grad_loss(depth_gt, depth_pred)
+    normals_loss = self.normals_loss(cur_data["normals_b3hw"], outputs["normals_pred_b3hw"])
+    mv_loss = self.mv_depth_loss(
+        depth_pred_b1hw=depth_pred,
+        cur_depth_b1hw=depth_gt,
+        src_depth_bk1hw=src_data["depth_b1hw"],
+        cur_invK_b44=cur_data["invK_s0_b44"],
+        src_K_bk44=src_data["K_s0_b44"],
+        cur_world_T_cam_b44=cur_data["world_T_cam_b44"],
+        src_cam_T_world_bk44=src_data["cam_T_world_b44"],
+    )
+    loss = terms["ms_loss"] + 1.0 * grad_loss + 1.0 * normals_loss + 0.2 * mv_loss
+    return {
+        "loss": loss,
+        "si_loss": terms["si_loss"],
+        "grad_loss": grad_loss,
+        "abs_loss": terms["abs_loss"],
+        "normals_loss": normals_loss,
+        "ms_loss": terms["ms_loss"],
+        "inv_abs_loss": terms["inv_abs_loss"],
+        "log_l1_loss": terms["log_l1_loss"],
+        "mv_loss": mv_loss,
+    }

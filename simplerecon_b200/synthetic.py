@@ -344,3 +344,42 @@ def make_normals_batch(seed: int = 0, batch: int = 2, height: int = 48, width: i
             zy, zx = torch.randint(0, height, (1,), generator=g).item(), torch.randint(0, width, (1,), generator=g).item()
             gt[b, 0, zy:zy + max(1, height // 8), zx:zx + max(1, width // 8)] = 0.0
     return dict(depth_gt_b1hw=gt, depth_pred_b1hw=pred, invK_b44=torch.inverse(K4))
+
+
+def make_training_step_batch(seed: int = 0, B: int = 2, H: int = 48, W: int = 64, views: int = 3,
+                             normal_generator=None) -> tuple[dict, dict, dict]:
+    """``(cur_data, src_data, outputs)`` of one training step as ``DepthModel.compute_losses`` reads them
+    (reference experiment_modules/depth_model.py:439-485), on the CPU: the scenes, cameras and source depths of
+    ``make_mvloss_batch``; a ground truth with NaN holes (a blob and isolated pixels) and ``mask_b`` =
+    ``depth > 1e-3 & depth < 10`` with NaN outside it, as the datasets build them (datasets/scannet_dataset.py:508-513);
+    four decoder scales ``log_depth_pred_s{i}_b1hw`` at (H >> i) x (W >> i), the log of the noisy prediction
+    average-pooled to that size plus noise; and ``depth_pred_s0_b1hw = exp(s0)``.  With ``normal_generator``
+    (a ``NormalGenerator``) the normals ``step`` adds (:526-531) are computed from the ground truth and from
+    ``depth_pred_s0``."""
+    t = make_mvloss_batch(seed=seed, batch=B, views=views, height=H, width=W)
+    g = torch.Generator().manual_seed(6161 + seed)
+    gt = t["cur_depth_b1hw"]
+    gt = torch.where(gt > 0, gt, torch.roll(gt, 1, -1))             # undo the scan's scattered zeroed pixels
+    v, u = torch.meshgrid(torch.arange(H), torch.arange(W), indexing="ij")
+    for b in range(B):
+        cy, cx = torch.randint(0, H, (1,), generator=g).item(), torch.randint(0, W, (1,), generator=g).item()
+        r = max(1.0, min(H, W) / 8)
+        gt[b, 0][(v - cy) ** 2 + (u - cx) ** 2 <= r * r] = float("nan")
+        gt[b, 0].view(-1)[torch.randint(0, H * W, (2,), generator=g)] = float("nan")
+    mask_b = (gt > 1e-3) & (gt < 10.0)
+    gt[~mask_b] = float("nan")
+    log_pred = torch.log(t["depth_pred_b1hw"])
+    outputs = {}
+    for i in range(4):
+        h, w = max(1, H >> i), max(1, W >> i)
+        s = torch.nn.functional.adaptive_avg_pool2d(log_pred, (h, w)) if i else log_pred
+        outputs[f"log_depth_pred_s{i}_b1hw"] = (s + 0.02 * i * torch.randn(B, 1, h, w, generator=g)).contiguous()
+    outputs["depth_pred_s0_b1hw"] = torch.exp(outputs["log_depth_pred_s0_b1hw"])
+    cur_data = {"depth_b1hw": gt, "mask_b_b1hw": mask_b, "mask_b1hw": mask_b.float(),
+                "invK_s0_b44": t["cur_invK_b44"], "world_T_cam_b44": t["cur_world_T_cam_b44"]}
+    src_data = {"depth_b1hw": t["src_depth_bk1hw"], "K_s0_b44": t["src_K_bk44"],
+                "cam_T_world_b44": t["src_cam_T_world_bk44"]}
+    if normal_generator is not None:
+        cur_data["normals_b3hw"] = normal_generator(gt, cur_data["invK_s0_b44"])
+        outputs["normals_pred_b3hw"] = normal_generator(outputs["depth_pred_s0_b1hw"], cur_data["invK_s0_b44"])
+    return cur_data, src_data, outputs
