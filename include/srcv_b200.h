@@ -362,6 +362,66 @@ int32_t srcv_mesh_extract_color(const srcv_mesh_args* args, const void* colors, 
                                 float* vert_colors, int32_t* faces, int64_t V, int64_t F, void* workspace,
                                 size_t workspace_bytes, void* stream);
 
+/* ---- the voxel-block hashed TSDF volume (SparseTSDF, DESIGN §4.16) -------------------- *
+ * The dense volume's lattice (voxel i at origin + i * voxel_size, any integer i) stored as 8^3-voxel
+ * blocks, allocated where some frame can change a voxel: values, weights and colours read back bitwise
+ * equal to a dense volume on the same lattice fed the same frames, wherever that volume lies.
+ *   state        DEVICE, srcv_sparse_tsdf_state_bytes() bytes, 256-byte aligned, owned by the caller:
+ *                a header of SRCV_SPARSE_HDR_WORDS uint32 words at offset 0, then the hash table (a
+ *                power of two >= 2 max_blocks slots), the pool of max_blocks blocks (fp16 values and
+ *                weights, 1 KiB each; 6 KiB of fp32 colour planes more when `color`)
+ *   max_blocks   pool capacity in blocks, 1 .. 2^26
+ * Header words: BLOCKS = blocks requested so far (it keeps counting past max_blocks, so after an overflow
+ * it is the capacity needed), LOST = inserts that found the hash table full, RANGE = non-zero if a frame
+ * reached outside the +-2^23-voxel lattice or had a singular projection.  The state is valid while
+ * BLOCKS <= max_blocks and LOST == RANGE == 0; nothing here synchronises to check it.
+ * srcv_sparse_tsdf_reset initialises the state (1 launch).  The integrate calls take the dense calls'
+ * frames, workspace sizing rule (srcv_sparse_tsdf_workspace_bytes) and colour descriptor (its `colors`
+ * is ignored: the colour planes are in the state): 4 launches per <= 16 frames.
+ * Mesh extraction is srcv_mesh_*'s mesh (DESIGN §4.10) on the unbounded lattice, in index space
+ * relative to `origin`: srcv_sparse_tsdf_mesh_begin(blocks = BLOCKS) adds the unallocated blocks just
+ * below allocated ones (re-read BLOCKS: allocated + boundary, which must fit max_blocks), then
+ * srcv_sparse_tsdf_mesh_count / _extract with args->blocks = that count, as srcv_mesh_count / _extract
+ * (vert_colors NULL: no colours), then srcv_sparse_tsdf_mesh_end(blocks = the first BLOCKS) restores the
+ * table.  srcv_sparse_tsdf_read_box writes the (X,Y,Z) = dims box starting at lattice voxel lo as dense
+ * fp16 values / weights (and (3,X,Y,Z) f32 colours, or NULL), -1 / 0 / 0 where nothing is allocated. */
+#define SRCV_SPARSE_HDR_BLOCKS 0
+#define SRCV_SPARSE_HDR_LOST 1
+#define SRCV_SPARSE_HDR_RANGE 2
+#define SRCV_SPARSE_HDR_WORDS 4
+typedef struct srcv_sparse_tsdf {
+  void* state;
+  int32_t max_blocks;
+  int32_t color;            /* 1: the state holds colour planes */
+  float origin[3];
+  float voxel_size;
+  float truncation_voxels;
+  float max_weight;
+} srcv_sparse_tsdf;
+typedef struct srcv_sparse_mesh_args {
+  int32_t blocks;           /* allocated + boundary blocks, read back after srcv_sparse_tsdf_mesh_begin */
+  float origin[3];          /* already fp16-rounded, as srcv_mesh_args */
+  int32_t scale_to_world, single_mesh;
+} srcv_sparse_mesh_args;
+size_t srcv_sparse_tsdf_state_bytes(const srcv_sparse_tsdf* volume);
+int32_t srcv_sparse_tsdf_reset(const srcv_sparse_tsdf* volume, void* stream);
+size_t srcv_sparse_tsdf_workspace_bytes(const srcv_tsdf_frames* frames);
+int32_t srcv_sparse_tsdf_integrate_f16(const srcv_sparse_tsdf* volume, const srcv_tsdf_frames* frames,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_sparse_tsdf_integrate_color_f16(const srcv_sparse_tsdf* volume, const srcv_tsdf_frames* frames,
+                                             const srcv_tsdf_color* color, void* workspace, size_t workspace_bytes,
+                                             void* stream);
+int32_t srcv_sparse_tsdf_mesh_begin(const srcv_sparse_tsdf* volume, int32_t blocks, void* stream);
+int32_t srcv_sparse_tsdf_mesh_end(const srcv_sparse_tsdf* volume, int32_t blocks, void* stream);
+size_t srcv_sparse_tsdf_mesh_workspace_bytes(const srcv_sparse_mesh_args* args);
+int32_t srcv_sparse_tsdf_mesh_count(const srcv_sparse_tsdf* volume, const srcv_sparse_mesh_args* args, int64_t* counts,
+                                    void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_sparse_tsdf_mesh_extract(const srcv_sparse_tsdf* volume, const srcv_sparse_mesh_args* args, float* verts,
+                                      float* normals, float* vert_colors, int32_t* faces, int64_t V, int64_t F,
+                                      void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* volume, const int32_t lo[3], const int32_t dims[3],
+                                  void* values, void* weights, void* colors, void* stream);
+
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py
  * :12-97), which pc_fusion.py:158 runs for every frame of a scan against all the others: for each

@@ -19,7 +19,7 @@ __all__ = [
     "BackprojectDepth", "Project3D", "pose_distance", "install", "uninstall",
 ]
 __version__ = "0.1.0"
-from .tsdf import TSDF, TSDFFuser  # noqa: E402,F401  (reference tools/tsdf.py)
+from .tsdf import SparseTSDF, TSDF, TSDFFuser  # noqa: E402,F401  (reference tools/tsdf.py; SparseTSDF: DESIGN §4.16)
 from .fusers import ColorFuser  # noqa: E402,F401  (OurFuser with colour, DESIGN §4.11)
 from . import point_cloud_fusion  # noqa: E402,F401  (reference tools/torch_point_cloud_fusion.py)
 from .losses import MSGradientLoss, MVDepthLoss, ScaleInvariantLoss  # noqa: E402,F401  (reference losses.py:11-54, :79-208)

@@ -77,6 +77,19 @@ class MeshArgs(C.Structure):
                 ("single_mesh", C.c_int32)]
 
 
+class SparseTsdf(C.Structure):
+    _fields_ = [("state", _fp), ("max_blocks", C.c_int32), ("color", C.c_int32), ("origin", C.c_float * 3),
+                ("voxel_size", C.c_float), ("truncation_voxels", C.c_float), ("max_weight", C.c_float)]
+
+
+class SparseMeshArgs(C.Structure):
+    _fields_ = [("blocks", C.c_int32), ("origin", C.c_float * 3), ("scale_to_world", C.c_int32),
+                ("single_mesh", C.c_int32)]
+
+
+SPARSE_HDR_BLOCKS, SPARSE_HDR_LOST, SPARSE_HDR_RANGE, SPARSE_HDR_WORDS = 0, 1, 2, 4
+
+
 class MvsScan(C.Structure):
     _fields_ = [("depths", _fp), ("K", _fp), ("K_inv", _fp), ("cam_T_world", _fp), ("world_T_cam", _fp),
                 ("N", C.c_int32), ("H", C.c_int32), ("W", C.c_int32)]
@@ -146,6 +159,20 @@ SYMBOLS = {
     "srcv_mesh_extract": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, _fp, C.c_int64, C.c_int64, _fp, C.c_size_t, _fp]),
     "srcv_mesh_extract_color": (C.c_int32, [C.POINTER(MeshArgs), _fp, _fp, _fp, _fp, _fp, C.c_int64, C.c_int64, _fp,
                                             C.c_size_t, _fp]),
+    "srcv_sparse_tsdf_state_bytes": (C.c_size_t, [C.POINTER(SparseTsdf)]),
+    "srcv_sparse_tsdf_reset": (C.c_int32, [C.POINTER(SparseTsdf), _fp]),
+    "srcv_sparse_tsdf_workspace_bytes": (C.c_size_t, [C.POINTER(TsdfFrames)]),
+    "srcv_sparse_tsdf_integrate_f16": (C.c_int32, [C.POINTER(SparseTsdf), C.POINTER(TsdfFrames), _fp, C.c_size_t, _fp]),
+    "srcv_sparse_tsdf_integrate_color_f16": (C.c_int32, [C.POINTER(SparseTsdf), C.POINTER(TsdfFrames),
+                                                         C.POINTER(TsdfColor), _fp, C.c_size_t, _fp]),
+    "srcv_sparse_tsdf_mesh_begin": (C.c_int32, [C.POINTER(SparseTsdf), C.c_int32, _fp]),
+    "srcv_sparse_tsdf_mesh_end": (C.c_int32, [C.POINTER(SparseTsdf), C.c_int32, _fp]),
+    "srcv_sparse_tsdf_mesh_workspace_bytes": (C.c_size_t, [C.POINTER(SparseMeshArgs)]),
+    "srcv_sparse_tsdf_mesh_count": (C.c_int32, [C.POINTER(SparseTsdf), C.POINTER(SparseMeshArgs), _fp, _fp, C.c_size_t,
+                                                _fp]),
+    "srcv_sparse_tsdf_mesh_extract": (C.c_int32, [C.POINTER(SparseTsdf), C.POINTER(SparseMeshArgs), _fp, _fp, _fp, _fp,
+                                                  C.c_int64, C.c_int64, _fp, C.c_size_t, _fp]),
+    "srcv_sparse_tsdf_read_box": (C.c_int32, [C.POINTER(SparseTsdf), C.c_int32 * 3, C.c_int32 * 3, _fp, _fp, _fp, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

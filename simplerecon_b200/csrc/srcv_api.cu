@@ -552,6 +552,158 @@ int32_t srcv_mesh_extract_color(const srcv_mesh_args* a, const void* colors, flo
                       workspace_bytes, stream_);
 }
 
+static int32_t check_sparse(const srcv_sparse_tsdf* v) {
+  if (!v) return fail(SRCV_ERR_NULL, "sparse volume descriptor is NULL");
+  if (!v->state) return fail(SRCV_ERR_NULL, "state is NULL");
+  if (v->max_blocks < 1 || v->max_blocks > (1 << 26))
+    return fail(SRCV_ERR_SHAPE, "max_blocks = %d out of range (1 .. 2^26)", v->max_blocks);
+  if (!(v->voxel_size > 0.f) || !(v->truncation_voxels > 0.f) || !(v->max_weight > 0.f))
+    return fail(SRCV_ERR_SHAPE, "voxel_size, truncation and max_weight must be positive");
+  if ((reinterpret_cast<uintptr_t>(v->state) & 255u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "state must be 256-byte aligned");
+  return SRCV_OK;
+}
+
+size_t srcv_sparse_tsdf_state_bytes(const srcv_sparse_tsdf* v) {
+  if (!v || v->max_blocks < 1 || v->max_blocks > (1 << 26)) return 0;
+  return sparse_tsdf_state_bytes(*v);
+}
+
+int32_t srcv_sparse_tsdf_reset(const srcv_sparse_tsdf* v, void* stream_) {
+  if (int32_t e = check_sparse(v)) return e;
+  g_last_variant.store("sparse_tsdf_reset");
+  cudaError_t err = launch_sparse_tsdf_reset(*v, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_reset");
+  return SRCV_OK;
+}
+
+size_t srcv_sparse_tsdf_workspace_bytes(const srcv_tsdf_frames* f) {
+  if (!f || f->B <= 0 || f->H <= 0 || f->W <= 0) return 0;
+  return sparse_tsdf_workspace_bytes(*f);
+}
+
+static int32_t check_sparse_frames(const srcv_sparse_tsdf* v, const srcv_tsdf_frames* f, void* workspace,
+                                   size_t workspace_bytes) {
+  if (int32_t e = check_sparse(v)) return e;
+  if (!f) return fail(SRCV_ERR_NULL, "frames descriptor is NULL");
+  if (!f->depth || !f->cam_T_world || !f->K) return fail(SRCV_ERR_NULL, "depth / cam_T_world / K is NULL");
+  if (f->B <= 0 || f->H <= 0 || f->W <= 0 || f->W > 2048 || f->H > 2048)
+    return fail(SRCV_ERR_SHAPE, "bad frame batch B=%d H=%d W=%d (image sizes up to 2048 are exact in fp16)", f->B, f->H, f->W);
+  if (!(f->max_depth > f->min_depth)) return fail(SRCV_ERR_SHAPE, "max_depth must exceed min_depth");
+  if (((reinterpret_cast<uintptr_t>(f->depth) | reinterpret_cast<uintptr_t>(f->cam_T_world) |
+        reinterpret_cast<uintptr_t>(f->K)) & 1u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
+  return check_workspace(workspace, workspace_bytes, sparse_tsdf_workspace_bytes(*f));
+}
+
+int32_t srcv_sparse_tsdf_integrate_f16(const srcv_sparse_tsdf* v, const srcv_tsdf_frames* f, void* workspace,
+                                       size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_sparse_frames(v, f, workspace, workspace_bytes)) return e;
+  g_last_variant.store("sparse_tsdf_integrate_f16");
+  cudaError_t err = launch_sparse_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_integrate");
+  return SRCV_OK;
+}
+
+int32_t srcv_sparse_tsdf_integrate_color_f16(const srcv_sparse_tsdf* v, const srcv_tsdf_frames* f,
+                                             const srcv_tsdf_color* c, void* workspace, size_t workspace_bytes,
+                                             void* stream_) {
+  if (!c) return fail(SRCV_ERR_NULL, "colour descriptor is NULL");
+  if (!c->images) return fail(SRCV_ERR_NULL, "images is NULL");
+  if (int32_t e = check_sparse_frames(v, f, workspace, workspace_bytes)) return e;
+  if (!v->color) return fail(SRCV_ERR_UNSUPPORTED, "this sparse volume has no colour planes");
+  if (c->Hc < 1 || c->Wc < 1 || (long long)c->Hc * c->Wc > (1ll << 30))
+    return fail(SRCV_ERR_SHAPE, "bad colour image size Hc=%d Wc=%d", c->Hc, c->Wc);
+  for (int ch = 0; ch < 3; ++ch)
+    if (!(c->std[ch] != 0.f)) return fail(SRCV_ERR_SHAPE, "colour std[%d] must be non-zero", ch);
+  if ((reinterpret_cast<uintptr_t>(c->images) & 3u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "images must be 4-byte aligned");
+  g_last_variant.store("sparse_tsdf_integrate_color_f16");
+  cudaError_t err = launch_sparse_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_), c);
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_integrate_color");
+  return SRCV_OK;
+}
+
+int32_t srcv_sparse_tsdf_mesh_begin(const srcv_sparse_tsdf* v, int32_t blocks, void* stream_) {
+  if (int32_t e = check_sparse(v)) return e;
+  if (blocks < 0 || blocks > v->max_blocks) return fail(SRCV_ERR_SHAPE, "blocks = %d outside 0 .. max_blocks", blocks);
+  g_last_variant.store("sparse_tsdf_mesh");
+  cudaError_t err = launch_sparse_mesh_begin(*v, blocks, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_mesh_begin");
+  return SRCV_OK;
+}
+
+int32_t srcv_sparse_tsdf_mesh_end(const srcv_sparse_tsdf* v, int32_t blocks, void* stream_) {
+  if (int32_t e = check_sparse(v)) return e;
+  if (blocks < 0 || blocks > v->max_blocks) return fail(SRCV_ERR_SHAPE, "blocks = %d outside 0 .. max_blocks", blocks);
+  cudaError_t err = launch_sparse_mesh_end(*v, blocks, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_mesh_end");
+  return SRCV_OK;
+}
+
+size_t srcv_sparse_tsdf_mesh_workspace_bytes(const srcv_sparse_mesh_args* a) {
+  if (!a || a->blocks < 0) return 0;
+  return sparse_mesh_workspace_bytes(*a);
+}
+
+static int32_t check_sparse_mesh(const srcv_sparse_tsdf* v, const srcv_sparse_mesh_args* a, void* workspace,
+                                 size_t workspace_bytes) {
+  if (int32_t e = check_sparse(v)) return e;
+  if (!a) return fail(SRCV_ERR_NULL, "mesh arguments are NULL");
+  if (a->blocks < 0 || a->blocks > v->max_blocks)
+    return fail(SRCV_ERR_SHAPE, "blocks = %d outside 0 .. max_blocks = %d", a->blocks, v->max_blocks);
+  return check_workspace(workspace, workspace_bytes, sparse_mesh_workspace_bytes(*a));
+}
+
+int32_t srcv_sparse_tsdf_mesh_count(const srcv_sparse_tsdf* v, const srcv_sparse_mesh_args* a, int64_t* counts,
+                                    void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_sparse_mesh(v, a, workspace, workspace_bytes)) return e;
+  if (!counts) return fail(SRCV_ERR_NULL, "counts is NULL");
+  g_last_variant.store("sparse_tsdf_mesh_mc");
+  cudaError_t err = launch_sparse_mesh_count(*v, *a, reinterpret_cast<long long*>(counts), workspace,
+                                             static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_mesh_count");
+  return SRCV_OK;
+}
+
+int32_t srcv_sparse_tsdf_mesh_extract(const srcv_sparse_tsdf* v, const srcv_sparse_mesh_args* a, float* verts,
+                                      float* normals, float* vert_colors, int32_t* faces, int64_t V, int64_t F,
+                                      void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_sparse_mesh(v, a, workspace, workspace_bytes)) return e;
+  if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
+  if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
+  if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
+  if (vert_colors && !v->color) return fail(SRCV_ERR_UNSUPPORTED, "vertex colours need a volume with colour planes");
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  long long totals[2] = {-1, -1};
+  cudaError_t err = sparse_mesh_read_totals(*a, workspace, totals, stream);
+  if (err != cudaSuccess) return cuda_fail(err, "sparse mesh totals");
+  if (totals[0] != V || totals[1] != F)
+    return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match srcv_sparse_tsdf_mesh_count (%lld, %lld) for this workspace",
+                (long long)V, (long long)F, totals[0], totals[1]);
+  g_last_variant.store(vert_colors ? "sparse_tsdf_mesh_mc_color" : "sparse_tsdf_mesh_mc");
+  err = launch_sparse_mesh_extract(*v, *a, verts, normals, vert_colors, faces, workspace, stream);
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_mesh_extract");
+  return SRCV_OK;
+}
+
+int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* v, const int32_t lo[3], const int32_t dims[3], void* values,
+                                  void* weights, void* colors, void* stream_) {
+  if (int32_t e = check_sparse(v)) return e;
+  if (!lo || !dims || !values || !weights) return fail(SRCV_ERR_NULL, "lo / dims / values / weights is NULL");
+  if (colors && !v->color) return fail(SRCV_ERR_UNSUPPORTED, "colours need a volume with colour planes");
+  if (dims[0] < 1 || dims[1] < 1 || dims[2] < 1 || (long long)dims[0] * dims[1] * dims[2] > (1ll << 40))
+    return fail(SRCV_ERR_SHAPE, "bad box %d x %d x %d", dims[0], dims[1], dims[2]);
+  for (int a = 0; a < 3; ++a)
+    if ((long long)lo[a] < -(8ll << 20) || (long long)lo[a] + dims[a] > (8ll << 20))
+      return fail(SRCV_ERR_SHAPE, "box outside the +-2^23-voxel lattice");
+  if (((reinterpret_cast<uintptr_t>(values) | reinterpret_cast<uintptr_t>(weights)) & 1u) != 0 ||
+      (reinterpret_cast<uintptr_t>(colors) & 3u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "misaligned output arrays");
+  g_last_variant.store("sparse_tsdf_read_box");
+  cudaError_t err = launch_sparse_tsdf_read_box(*v, lo, dims, values, weights, colors, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_read_box");
+  return SRCV_OK;
+}
+
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {
   if (!s || s->N <= 0) return 0;
   return mvs_workspace_bytes(s->N);

@@ -114,6 +114,25 @@ cudaError_t launch_mesh_extract(const srcv_mesh_args& a, float* verts, float* no
                                 void* workspace, cudaStream_t stream, const float* colors = nullptr,
                                 float* vert_colors = nullptr);
 
+// the voxel-block hashed TSDF volume (csrc/srcv_tsdf_sparse.cuh, in the srcv_tsdf.cu unit)
+size_t sparse_tsdf_state_bytes(const srcv_sparse_tsdf& v);
+size_t sparse_tsdf_workspace_bytes(const srcv_tsdf_frames& f);
+cudaError_t launch_sparse_tsdf_reset(const srcv_sparse_tsdf& v, cudaStream_t stream);
+cudaError_t launch_sparse_tsdf_integrate(const srcv_sparse_tsdf& v, const srcv_tsdf_frames& f, void* workspace,
+                                         cudaStream_t stream, const srcv_tsdf_color* color = nullptr);
+cudaError_t launch_sparse_tsdf_read_box(const srcv_sparse_tsdf& v, const int lo[3], const int dims[3], void* values,
+                                        void* weights, void* colors, cudaStream_t stream);
+cudaError_t launch_sparse_mesh_begin(const srcv_sparse_tsdf& v, int blocks, cudaStream_t stream);
+cudaError_t launch_sparse_mesh_end(const srcv_sparse_tsdf& v, int blocks, cudaStream_t stream);
+size_t sparse_mesh_workspace_bytes(const srcv_sparse_mesh_args& a);
+cudaError_t launch_sparse_mesh_count(const srcv_sparse_tsdf& v, const srcv_sparse_mesh_args& a, long long* counts,
+                                     void* workspace, cudaStream_t stream);
+cudaError_t sparse_mesh_read_totals(const srcv_sparse_mesh_args& a, void* workspace, long long totals[2],
+                                    cudaStream_t stream);
+cudaError_t launch_sparse_mesh_extract(const srcv_sparse_tsdf& v, const srcv_sparse_mesh_args& a, float* verts,
+                                       float* normals, float* vert_colors, int32_t* faces, void* workspace,
+                                       cudaStream_t stream);
+
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);
 cudaError_t launch_mvs_consistency(const srcv_mvs_scan& s, int ref, float z_thresh, int n_consistent,

@@ -33,7 +33,9 @@
 // output is deterministic and canonically ordered.
 //
 // This file is compiled as part of srcv_tsdf.cu's translation unit (included at its end): the
-// TSDF unit holds both operations on the fused volume, integration and mesh extraction.
+// TSDF unit holds both operations on the fused volume, integration and mesh extraction.  The helpers
+// and kernels are templates over the volume they read (MeshParams here; the voxel-block view of
+// srcv_tsdf_sparse.cuh, which instantiates the same kernels on an unbounded lattice).
 #pragma once
 #include "srcv_kernels.h"
 #ifdef SRCV_HOST_EMU
@@ -71,26 +73,39 @@ __device__ __forceinline__ float ld(const MeshParams& p, int x, int y, int z) {
 
 __device__ __forceinline__ int dim(const MeshParams& p, int a) { return a == 0 ? p.X : (a == 1 ? p.Y : p.Z); }
 
+// The voxel access the helpers and kernels below are written against, so that the voxel-block volume
+// (srcv_tsdf_sparse.cuh) runs the same code with its own overloads: the weight, the bounds of the lattice,
+// and the index of a voxel's slot in the per-voxel arrays (vbase, colour planes).
+__device__ __forceinline__ float wt(const MeshParams& p, int x, int y, int z) { return __half2float(p.w[vidx(p, x, y, z)]); }
+__device__ __forceinline__ bool cube_exists(const MeshParams& p, int x, int y, int z) {
+  return !(x < 0 || y < 0 || z < 0 || x >= p.X - 1 || y >= p.Y - 1 || z >= p.Z - 1);
+}
+__device__ __forceinline__ bool has_next(const MeshParams& p, int a, int c) { return c + 1 < dim(p, a); }
+__device__ __forceinline__ bool at_low(const MeshParams&, int, int c) { return c == 0; }
+__device__ __forceinline__ bool at_high(const MeshParams& p, int a, int c) { return c == dim(p, a) - 1; }
+
 __device__ __forceinline__ int popc3(unsigned m) { return (int)(m & 1u) + (int)((m >> 1) & 1u) + (int)((m >> 2) & 1u); }
 
 // the cube anchored at (x,y,z) exists and is processed
-__device__ __forceinline__ bool cube_ok(const MeshParams& p, int x, int y, int z) {
-  if (x < 0 || y < 0 || z < 0 || x >= p.X - 1 || y >= p.Y - 1 || z >= p.Z - 1) return false;
+template <class P>
+__device__ __forceinline__ bool cube_ok(const P& p, int x, int y, int z) {
+  if (!cube_exists(p, x, y, z)) return false;
   if (!p.single) return true;
 #pragma unroll
   for (int c = 0; c < 8; ++c)
-    if (!(__half2float(p.w[vidx(p, x + (c & 1), y + ((c >> 1) & 1), z + (c >> 2))]) > 0.0f)) return false;
+    if (!(wt(p, x + (c & 1), y + ((c >> 1) & 1), z + (c >> 2)) > 0.0f)) return false;
   return true;
 }
 
 // bit a: the edge along axis a from (x,y,z) crosses the level and is emitted
-__device__ __forceinline__ unsigned owned_edges(const MeshParams& p, int x, int y, int z) {
+template <class P>
+__device__ __forceinline__ unsigned owned_edges(const P& p, int x, int y, int z) {
   const bool in0 = ld(p, x, y, z) < 0.0f;
   unsigned m = 0;
 #pragma unroll
   for (int a = 0; a < 3; ++a) {
     const int c = a == 0 ? x : (a == 1 ? y : z);
-    if (c + 1 >= dim(p, a)) continue;
+    if (!has_next(p, a, c)) continue;
     if ((ld(p, x + (a == 0), y + (a == 1), z + (a == 2)) < 0.0f) == in0) continue;
     if (p.single) {
       // the (up to) four cubes that contain the edge: anchors owner - {0,1} e_b - {0,1} e_c
@@ -111,7 +126,8 @@ __device__ __forceinline__ unsigned owned_edges(const MeshParams& p, int x, int 
 __device__ __forceinline__ float edge_t(float va, float vb) { return __fdiv_rn(-va, __fadd_rn(vb, -va)); }
 
 // inside-mask of the cube anchored at (x,y,z), and its 8 corner values
-__device__ __forceinline__ unsigned cube_case(const MeshParams& p, int x, int y, int z, float v[8]) {
+template <class P>
+__device__ __forceinline__ unsigned cube_case(const P& p, int x, int y, int z, float v[8]) {
   unsigned cs = 0;
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
@@ -157,8 +173,9 @@ __device__ __forceinline__ bool same_point(const float a[3], const float b[3]) {
 }
 
 // bit k: triangle k of the cube's case is kept (not degenerate); 0 if the cube is not processed
-__device__ __forceinline__ unsigned kept_tris(const MeshParams& p, int x, int y, int z, float v[8], unsigned& cs) {
-  if (x >= p.X - 1 || y >= p.Y - 1 || z >= p.Z - 1) return 0u;
+template <class P>
+__device__ __forceinline__ unsigned kept_tris(const P& p, int x, int y, int z, float v[8], unsigned& cs) {
+  if (!cube_exists(p, x, y, z)) return 0u;
   cs = cube_case(p, x, y, z, v);
   if (cs == 0u || cs == 255u || !cube_ok(p, x, y, z)) return 0u;
   unsigned keep = 0;
@@ -260,8 +277,12 @@ __device__ Chunk chunk_of(const MeshParams& p) {
   return c;
 }
 
-template <int VEC>
-__device__ void chunk_counts(const MeshParams& p, const Chunk& c, int& nv, int& nf) {
+// the dense volume is its own view; a voxel's slot in the per-voxel arrays is its linear index
+__device__ __forceinline__ const MeshParams& view_of(const MeshParams& p, const Chunk&) { return p; }
+__device__ __forceinline__ size_t vslot(const MeshParams& p, int x, int y, int z) { return vidx(p, x, y, z); }
+
+template <int VEC, class P, class C>
+__device__ void chunk_counts(const P& p, const C& c, int& nv, int& nf) {
   nv = 0;
   nf = 0;
   if (!c.live) return;
@@ -275,11 +296,11 @@ __device__ void chunk_counts(const MeshParams& p, const Chunk& c, int& nv, int& 
 
 __device__ __forceinline__ unsigned block_linear() { return blockIdx.y * gridDim.x + blockIdx.x; }
 
-template <int VEC>
-__global__ void __launch_bounds__(kMeshThreads) mesh_count_kernel(MeshParams p, int* __restrict__ block_counts) {
-  const Chunk c = chunk_of<VEC>(p);
+template <int VEC, class P = MeshParams>
+__global__ void __launch_bounds__(kMeshThreads) mesh_count_kernel(P p, int* __restrict__ block_counts) {
+  const auto c = chunk_of<VEC>(p);
   int nv, nf, ta, tb;
-  chunk_counts<VEC>(p, c, nv, nf);
+  chunk_counts<VEC>(view_of(p, c), c, nv, nf);
   block_scan2(nv, nf, ta, tb);
   if (threadIdx.x == 0) {
     block_counts[2 * block_linear() + 0] = ta;
@@ -323,20 +344,22 @@ mesh_scan_kernel(const int* __restrict__ block_counts, long long nblocks, long l
   }
 }
 
-__device__ __forceinline__ float grad1(const MeshParams& p, int x, int y, int z, int a) {
-  const int c = a == 0 ? x : (a == 1 ? y : z), n = dim(p, a);
+template <class P>
+__device__ __forceinline__ float grad1(const P& p, int x, int y, int z, int a) {
+  const int c = a == 0 ? x : (a == 1 ? y : z);
   const int dx = a == 0, dy = a == 1, dz = a == 2;
-  if (c == 0) return __fadd_rn(ld(p, x + dx, y + dy, z + dz), -ld(p, x, y, z));
-  if (c == n - 1) return __fadd_rn(ld(p, x, y, z), -ld(p, x - dx, y - dy, z - dz));
+  if (at_low(p, a, c)) return __fadd_rn(ld(p, x + dx, y + dy, z + dz), -ld(p, x, y, z));
+  if (at_high(p, a, c)) return __fadd_rn(ld(p, x, y, z), -ld(p, x - dx, y - dy, z - dz));
   return __fmul_rn(__fadd_rn(ld(p, x + dx, y + dy, z + dz), -ld(p, x - dx, y - dy, z - dz)), 0.5f);
 }
 
-template <int VEC>
+template <int VEC, class P = MeshParams>
 __global__ void __launch_bounds__(kMeshThreads)
-mesh_vertex_kernel(MeshParams p, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
+mesh_vertex_kernel(P pp, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
                    int* __restrict__ vbase, float* __restrict__ verts, float* __restrict__ normals) {
   if (block_counts[2 * block_linear()] == 0) return;    // the whole block owns no vertex (block-uniform)
-  const Chunk c = chunk_of<VEC>(p);
+  const auto c = chunk_of<VEC>(pp);
+  decltype(auto) p = view_of(pp, c);      // the dense volume by reference, a block view by value
   int nv, nf, ta, tb;
   chunk_counts<VEC>(p, c, nv, nf);
   nf = 0;
@@ -347,7 +370,7 @@ mesh_vertex_kernel(MeshParams p, const int* __restrict__ block_counts, const lon
     const int x = c.x, y = c.y, z = c.z0 + i;
     const unsigned m = owned_edges(p, x, y, z);
     if (m == 0u) continue;
-    vbase[vidx(p, x, y, z)] = (int)off;
+    vbase[vslot(p, x, y, z)] = (int)off;
     const float v0 = ld(p, x, y, z);
     float g0[3];
 #pragma unroll
@@ -387,12 +410,13 @@ mesh_vertex_kernel(MeshParams p, const int* __restrict__ block_counts, const lon
 // endpoints observed (weight > 0): ca + t (cb - ca); one: its colour; none: grey 0.7.  Separately rounded
 // fp32 ops.  (Folded into the vertex pass, the colour state lives across the normals' IEEE-division
 // slow-path calls and ptxas spills it.)
-template <int VEC>
+template <int VEC, class P = MeshParams>
 __global__ void __launch_bounds__(kMeshThreads)
-mesh_vertex_color_kernel(MeshParams p, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
+mesh_vertex_color_kernel(P pp, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
                          const float* __restrict__ colors, size_t cplane, float* __restrict__ vert_colors) {
   if (block_counts[2 * block_linear()] == 0) return;    // the whole block owns no vertex (block-uniform)
-  const Chunk c = chunk_of<VEC>(p);
+  const auto c = chunk_of<VEC>(pp);
+  decltype(auto) p = view_of(pp, c);      // the dense volume by reference, a block view by value
   int nv, nf, ta, tb;
   chunk_counts<VEC>(p, c, nv, nf);
   nf = 0;
@@ -403,27 +427,26 @@ mesh_vertex_color_kernel(MeshParams p, const int* __restrict__ block_counts, con
     const int x = c.x, y = c.y, z = c.z0 + i;
     const unsigned m = owned_edges(p, x, y, z);
     if (m == 0u) continue;
-    const size_t ia = vidx(p, x, y, z);
     const float v0 = ld(p, x, y, z);
-    const bool oa = __half2float(p.w[ia]) > 0.0f;
+    const bool oa = wt(p, x, y, z) > 0.0f;
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
       if (!((m >> a) & 1u)) continue;
       const int qx = x + (a == 0), qy = y + (a == 1), qz = z + (a == 2);
-      const size_t ib = vidx(p, qx, qy, qz);
       const float t = edge_t(v0, ld(p, qx, qy, qz));           // the position's t (mesh_vertex_kernel)
-      const bool ob = __half2float(p.w[ib]) > 0.0f;
+      const bool ob = wt(p, qx, qy, qz) > 0.0f;
 #pragma unroll
       for (int ch = 0; ch < 3; ++ch) {
         const float* cc = colors + ch * cplane;
         float r = 0.7f;
+        // (a weighted voxel always has a slot: vslot is only asked for those)
         if (oa && ob) {
-          const float ca = cc[ia];
-          r = __fadd_rn(ca, __fmul_rn(t, __fadd_rn(cc[ib], -ca)));
+          const float ca = cc[vslot(p, x, y, z)];
+          r = __fadd_rn(ca, __fmul_rn(t, __fadd_rn(cc[vslot(p, qx, qy, qz)], -ca)));
         } else if (oa) {
-          r = cc[ia];
+          r = cc[vslot(p, x, y, z)];
         } else if (ob) {
-          r = cc[ib];
+          r = cc[vslot(p, qx, qy, qz)];
         }
         vert_colors[3 * off + ch] = r;
       }
@@ -432,12 +455,13 @@ mesh_vertex_color_kernel(MeshParams p, const int* __restrict__ block_counts, con
   }
 }
 
-template <int VEC>
+template <int VEC, class P = MeshParams>
 __global__ void __launch_bounds__(kMeshThreads)
-mesh_face_kernel(MeshParams p, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
+mesh_face_kernel(P pp, const int* __restrict__ block_counts, const long long* __restrict__ block_off,
                  const int* __restrict__ vbase, int* __restrict__ faces) {
   if (block_counts[2 * block_linear() + 1] == 0) return;   // the whole block anchors no face (block-uniform)
-  const Chunk c = chunk_of<VEC>(p);
+  const auto c = chunk_of<VEC>(pp);
+  decltype(auto) p = view_of(pp, c);      // the dense volume by reference, a block view by value
   int nv, nf, ta, tb;
   chunk_counts<VEC>(p, c, nv, nf);
   nv = 0;
@@ -459,7 +483,7 @@ mesh_face_kernel(MeshParams p, const int* __restrict__ block_counts, const long 
         edge_geom(mc::kTris[cs][3 * k + j], o, a);
         const int ox = x + o[0], oy = y + o[1], oz = z + o[2];
         const unsigned m = owned_edges(p, ox, oy, oz);
-        faces[3 * off + j] = vbase[vidx(p, ox, oy, oz)] + popc3(m & ((1u << a) - 1u));
+        faces[3 * off + j] = vbase[vslot(p, ox, oy, oz)] + popc3(m & ((1u << a) - 1u));
       }
       ++off;
     }

@@ -58,6 +58,13 @@ union Pack8 {
 
 __device__ __forceinline__ float r16(float x) { return __half2float(__float2half_rn(x)); }
 
+// the confidence of a depth sample ds (:264-266), in fp16 steps; the update is skipped unless it is > 0
+__device__ __forceinline__ float tsdf_confidence(const TsdfParams& p, float ds) {
+  float conf = r16(__fadd_rn(1.0f, -r16(__fdiv_rn(r16(__fadd_rn(ds, -p.min_depth)), p.depth_span))));
+  conf = fminf(fmaxf(conf, 0.0f), 1.0f);
+  return r16(__fmul_rn(conf, conf));
+}
+
 // (K @ E)[:3] in fp16: fp32 accumulation over j, one rounding (a half matmul in PyTorch)
 __global__ void tsdf_prep_kernel(const __half* __restrict__ K, const __half* __restrict__ E, int B,
                                  TsdfFrame* __restrict__ frames) {
@@ -81,20 +88,16 @@ struct TsdfColorParams {
   float mean[3], std[3];       // de-normalisation (x - mean) / std, then clamp to [0, 1]
 };
 
-// The kColor = false instantiation is the plain kernel: every colour statement is `if constexpr`.
+// The per-voxel update of one z column: VEC voxels at lattice indices (ix, iy, z0 .. z0+VEC-1) relative to
+// the origin, stored at tsdf[base ..] / weights[base ..] (and colour planes cp.plane apart), every frame of the
+// launch applied in order.  The dense kernel below and the voxel-block kernels (srcv_tsdf_sparse.cuh) both
+// run their voxels through this one function, so the two volumes compute the same bits.
+// The kColor = false instantiation is the plain update: every colour statement is `if constexpr`.
 template <int VEC, bool kColor>
 __device__ __forceinline__ void
-tsdf_integrate_body(const TsdfParams& p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
-                    const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights,
-                    const TsdfColorParams& cp) {
-  // grid.y walks x; grid.x * blockDim.x covers the (y, z-column) plane: 32-bit index arithmetic only
-  // (64-bit div/mod of a flat voxel index cost more than the projection of an empty column)
-  const unsigned zcols = (unsigned)(p.Z / VEC);
-  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= zcols * (unsigned)p.Y) return;
-  const int zc = (int)(t % zcols), iy = (int)(t / zcols), ix = (int)blockIdx.y;
-  const int z0 = zc * VEC;
-  const size_t base = ((size_t)ix * p.Y + iy) * p.Z + z0;
+tsdf_integrate_column(const TsdfParams& p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
+                      const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights,
+                      const TsdfColorParams& cp, int ix, int iy, int z0, size_t base) {
   // world coordinates: fp32 origin + index * voxel_size, then half (tools/tsdf.py:99-110, :92)
   const float wx = r16(__fadd_rn(p.ox, __fmul_rn((float)ix, p.voxel_size)));
   const float wy = r16(__fadd_rn(p.oy, __fmul_rn((float)iy, p.voxel_size)));
@@ -161,9 +164,7 @@ tsdf_integrate_body(const TsdfParams& p, const TsdfFrame* __restrict__ frames, c
       if (!(ds > 0.0f)) continue;
       const float dist = r16(__fadd_rn(ds, -vz));                  // :269
       if (!(dist > p.neg_trunc_h)) continue;
-      float conf = r16(__fadd_rn(1.0f, -r16(__fdiv_rn(r16(__fadd_rn(ds, -p.min_depth)), p.depth_span))));
-      conf = fminf(fmaxf(conf, 0.0f), 1.0f);
-      conf = r16(__fmul_rn(conf, conf));                           // :264-266
+      const float conf = tsdf_confidence(p, ds);                   // :264-266
       if (!(conf > 0.0f)) continue;
       const float nt = fminf(fmaxf(r16(__fdiv_rn(dist, p.trunc)), -1.0f), 1.0f);   // :270
       if (!loaded) {
@@ -249,6 +250,22 @@ tsdf_integrate_body(const TsdfParams& p, const TsdfFrame* __restrict__ frames, c
   }
 }
 
+template <int VEC, bool kColor>
+__device__ __forceinline__ void
+tsdf_integrate_body(const TsdfParams& p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
+                    const uint8_t* __restrict__ mask, __half* __restrict__ tsdf, __half* __restrict__ weights,
+                    const TsdfColorParams& cp) {
+  // grid.y walks x; grid.x * blockDim.x covers the (y, z-column) plane: 32-bit index arithmetic only
+  // (64-bit div/mod of a flat voxel index cost more than the projection of an empty column)
+  const unsigned zcols = (unsigned)(p.Z / VEC);
+  const unsigned t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= zcols * (unsigned)p.Y) return;
+  const int zc = (int)(t % zcols), iy = (int)(t / zcols), ix = (int)blockIdx.y;
+  const int z0 = zc * VEC;
+  const size_t base = ((size_t)ix * p.Y + iy) * p.Z + z0;
+  tsdf_integrate_column<VEC, kColor>(p, frames, depth, mask, tsdf, weights, cp, ix, iy, z0, base);
+}
+
 template <int VEC>
 __global__ void __launch_bounds__(256)
 tsdf_integrate_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const __half* __restrict__ depth,
@@ -264,6 +281,35 @@ tsdf_integrate_color_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, 
   tsdf_integrate_body<VEC, true>(p, frames, depth, mask, tsdf, weights, cp);
 }
 
+// the launch constants of frames b0 .. b0+nb-1 (shared by the dense and the voxel-block launchers)
+TsdfParams tsdf_params(const float origin[3], float voxel_size, float truncation_voxels, float max_weight,
+                       const srcv_tsdf_frames& f, int nb) {
+  const float trunc = truncation_voxels * voxel_size;
+  TsdfParams p;
+  p.X = 0; p.Y = 0; p.Z = 0; p.B = nb; p.H = f.H; p.W = f.W;
+  p.ox = origin[0]; p.oy = origin[1]; p.oz = origin[2]; p.voxel_size = voxel_size;
+  p.min_depth = f.min_depth;
+  p.depth_span = f.max_depth - f.min_depth;
+  p.trunc = trunc;
+  p.neg_trunc_h = -__half2float(__float2half_rn(trunc));
+  p.max_depth_h = __half2float(__float2half_rn(f.max_depth));
+  p.max_w = max_weight;
+  return p;
+}
+
+TsdfColorParams tsdf_color_params(const srcv_tsdf_color& color, float* colors, size_t plane, const srcv_tsdf_frames& f,
+                                  int b0) {
+  TsdfColorParams cp;
+  cp.colors = colors;
+  cp.plane = plane;
+  cp.Hc = color.Hc; cp.Wc = color.Wc;
+  cp.images = reinterpret_cast<const float*>(color.images) + (size_t)b0 * 3 * color.Hc * color.Wc;
+  cp.scale_x = (float)color.Wc / (float)f.W;
+  cp.scale_y = (float)color.Hc / (float)f.H;
+  for (int ch = 0; ch < 3; ++ch) { cp.mean[ch] = color.mean[ch]; cp.std[ch] = color.std[ch]; }
+  return cp;
+}
+
 }  // namespace
 
 size_t tsdf_workspace_bytes(int frames) { return sizeof(TsdfFrame) * (size_t)(frames < kMaxFrames ? frames : kMaxFrames) + 256; }
@@ -273,22 +319,14 @@ cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_fra
   TsdfFrame* frames = reinterpret_cast<TsdfFrame*>(workspace);
   __half* tsdf = reinterpret_cast<__half*>(v.tsdf_values);
   __half* weights = reinterpret_cast<__half*>(v.tsdf_weights);
-  const float trunc = v.truncation_voxels * v.voxel_size;
   for (int b0 = 0; b0 < f.B; b0 += kMaxFrames) {
     const int nb = (f.B - b0 < kMaxFrames) ? (f.B - b0) : kMaxFrames;
     const __half* K = reinterpret_cast<const __half*>(f.K) + (size_t)b0 * 16;
     const __half* E = reinterpret_cast<const __half*>(f.cam_T_world) + (size_t)b0 * 16;
     SRCV_LAUNCH(tsdf_prep_kernel, 1, 256, 0, stream, K, E, nb, frames);
     note_launch();
-    TsdfParams p;
-    p.X = v.X; p.Y = v.Y; p.Z = v.Z; p.B = nb; p.H = f.H; p.W = f.W;
-    p.ox = v.origin[0]; p.oy = v.origin[1]; p.oz = v.origin[2]; p.voxel_size = v.voxel_size;
-    p.min_depth = f.min_depth;
-    p.depth_span = f.max_depth - f.min_depth;
-    p.trunc = trunc;
-    p.neg_trunc_h = -__half2float(__float2half_rn(trunc));
-    p.max_depth_h = __half2float(__float2half_rn(f.max_depth));
-    p.max_w = v.max_weight;
+    TsdfParams p = tsdf_params(v.origin, v.voxel_size, v.truncation_voxels, v.max_weight, f, nb);
+    p.X = v.X; p.Y = v.Y; p.Z = v.Z;
     const __half* depth = reinterpret_cast<const __half*>(f.depth) + (size_t)b0 * f.H * f.W;
     const uint8_t* mask = f.depth_mask ? f.depth_mask + (size_t)b0 * f.H * f.W : nullptr;
     const uintptr_t cptr = color ? reinterpret_cast<uintptr_t>(color->colors) : 0;
@@ -297,14 +335,8 @@ cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_fra
     if (plane > 2147483647ll || v.X > 65535) return cudaErrorInvalidValue;
     const dim3 grid((unsigned)((plane + 255) / 256), (unsigned)v.X);
     if (color != nullptr) {
-      TsdfColorParams cp;
-      cp.colors = reinterpret_cast<float*>(color->colors);
-      cp.plane = (size_t)v.X * v.Y * v.Z;
-      cp.Hc = color->Hc; cp.Wc = color->Wc;
-      cp.images = reinterpret_cast<const float*>(color->images) + (size_t)b0 * 3 * color->Hc * color->Wc;
-      cp.scale_x = (float)color->Wc / (float)f.W;
-      cp.scale_y = (float)color->Hc / (float)f.H;
-      for (int ch = 0; ch < 3; ++ch) { cp.mean[ch] = color->mean[ch]; cp.std[ch] = color->std[ch]; }
+      const TsdfColorParams cp = tsdf_color_params(*color, reinterpret_cast<float*>(color->colors),
+                                                   (size_t)v.X * v.Y * v.Z, f, b0);
       if (vec) SRCV_LAUNCH(tsdf_integrate_color_kernel<kVec>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights, cp);
       else SRCV_LAUNCH(tsdf_integrate_color_kernel<1>, grid, 256, 0, stream, p, frames, depth, mask, tsdf, weights, cp);
     } else {
@@ -322,3 +354,6 @@ cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_fra
 
 // marching-cubes mesh extraction from the same volume (TSDF.to_mesh)
 #include "srcv_mesh.cuh"
+// the voxel-block hashed volume (SparseTSDF): integration through tsdf_integrate_column, meshing through
+// srcv_mesh.cuh's kernels
+#include "srcv_tsdf_sparse.cuh"

@@ -5,17 +5,20 @@ integration per frame); with its default ``ours`` fuser, ``--fuse_color`` prints
 colour (:197-207).  ``ColorFuser`` has ``OurFuser``'s interface and bounds logic and fuses the frames'
 colour into the kernel-backed volume (DESIGN §4.11); ``export_mesh`` writes a vertex-coloured binary PLY
 without trimesh.  ``install(fusion=True, fuse_color=True)`` makes ``get_fuser`` return it for
-``--depth_fuser ours --fuse_color``.
+``--depth_fuser ours --fuse_color``.  With ``unbounded=True`` and no ground-truth mesh its volume is a
+``SparseTSDF`` on the ±10 m cube's lattice instead of that cube (DESIGN §4.16), with or without colour;
+``install(fusion=True, unbounded_fusion=True)`` makes ``get_fuser`` use that for ``--depth_fuser ours``.
 """
 from __future__ import annotations
 
-from .tsdf import TSDF, TSDFFuser, colors_to_u8, write_ply
+from .tsdf import DEFAULT_BOUNDS, SparseTSDF, TSDF, TSDFFuser, colors_to_u8, write_ply
 
 
 class ColorFuser:
     """OurFuser's constructor, ``fuse_frames``, ``export_mesh`` and ``get_mesh``, with colour."""
 
-    def __init__(self, gt_path="", fusion_resolution=0.04, max_fusion_depth=3, fuse_color=True):
+    def __init__(self, gt_path="", fusion_resolution=0.04, max_fusion_depth=3, fuse_color=True, unbounded=False,
+                 max_blocks=1 << 17):
         self.fusion_resolution = fusion_resolution
         self.max_fusion_depth = max_fusion_depth
         self.fuse_color = bool(fuse_color)
@@ -23,9 +26,10 @@ class ColorFuser:
             import trimesh
             gt_mesh = trimesh.load(gt_path, force="mesh")
             tsdf_pred = TSDF.from_mesh(gt_mesh, voxel_size=fusion_resolution, color=self.fuse_color)
+        elif unbounded:                     # no bounds: voxel blocks where the frames reach, on the cube's lattice
+            tsdf_pred = SparseTSDF(fusion_resolution, max_blocks=max_blocks, color=self.fuse_color)
         else:                               # or a ±10 m cube (:51-60)
-            bounds = {"xmin": -10.0, "xmax": 10.0, "ymin": -10.0, "ymax": 10.0, "zmin": -10.0, "zmax": 10.0}
-            tsdf_pred = TSDF.from_bounds(bounds, voxel_size=fusion_resolution, color=self.fuse_color)
+            tsdf_pred = TSDF.from_bounds(dict(DEFAULT_BOUNDS), voxel_size=fusion_resolution, color=self.fuse_color)
         self.tsdf_fuser_pred = TSDFFuser(tsdf_pred, max_depth=max_fusion_depth)
 
     def fuse_frames(self, depths_b1hw, K_b44, cam_T_world_b44, color_b3hw):

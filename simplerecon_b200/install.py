@@ -12,6 +12,9 @@ the names ``tools.fusers_helper`` bound at import (tools/fusers_helper.py:8) if 
 imported.  ``install(fusion=True, fuse_color=True)`` also wraps ``tools.fusers_helper.get_fuser`` so that
 ``--depth_fuser ours --fuse_color`` gets a ``fusers.ColorFuser`` (colour fused on the GPU) instead of the
 reference's warning and a colourless ``OurFuser``; every other option goes to the original.
+``install(fusion=True, unbounded_fusion=True)`` wraps ``get_fuser`` so that ``--depth_fuser ours`` without a
+ground-truth mesh (every dataset but ScanNet) fuses into a ``SparseTSDF`` (DESIGN §4.16) instead of the dense
+±10 m cube, with ``--fuse_color`` or without; with a ground-truth mesh the dense path runs as before.
 ``install(metrics=True)`` swaps ``compute_depth_metrics`` / ``compute_depth_metrics_batched`` of
 ``utils.metrics_utils`` (and the name ``experiment_modules.depth_model`` binds at import, :16, if it was
 already imported) for wrappers that run CUDA tensors through the metrics kernel and hand anything else to
@@ -43,15 +46,18 @@ _saved: dict = {}
 
 def install(verbose: bool = False, losses: bool = False, fusion: bool = False, fuse_color: bool = False,
             metrics: bool = False, normals: bool = False, depth_losses: bool = False,
-            regression_losses: bool = False) -> list[str]:
+            regression_losses: bool = False, unbounded_fusion: bool = False) -> list[str]:
     """Returns the list of patched module names.  Requires the reference checkout to
     be importable (on ``sys.path``) as ``modules.cost_volume``; with ``losses=True`` also as ``losses``,
-    with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` also as ``tools.fusers_helper``,
+    with ``fusion=True`` also as ``tools.tsdf``, with ``fuse_color=True`` or ``unbounded_fusion=True`` also as
+    ``tools.fusers_helper``,
     with ``metrics=True`` also as ``utils.metrics_utils``, with ``normals=True`` also as ``losses`` and
     ``utils.geometry_utils``, with ``depth_losses=True`` also as ``losses``, with ``regression_losses=True``
     also as ``experiment_modules.depth_model``."""
     if fuse_color and not fusion:
         raise ValueError("install(fuse_color=True) needs fusion=True: colour is fused into the kernel-backed TSDF")
+    if unbounded_fusion and not fusion:
+        raise ValueError("install(unbounded_fusion=True) needs fusion=True: the volume is the kernel-backed SparseTSDF")
     from . import cost_volume as ours
     patched = []
     ref_cv = importlib.import_module("modules.cost_volume")
@@ -79,7 +85,8 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
     if fusion:
         from . import tsdf as ours_tsdf
         ref_tsdf = importlib.import_module("tools.tsdf")
-        fh = importlib.import_module("tools.fusers_helper") if fuse_color else sys.modules.get("tools.fusers_helper")
+        wrap = fuse_color or unbounded_fusion
+        fh = importlib.import_module("tools.fusers_helper") if wrap else sys.modules.get("tools.fusers_helper")
         for mod in [ref_tsdf] + ([fh] if fh is not None else []):
             for n in ("TSDF", "TSDFFuser"):
                 if hasattr(mod, n):
@@ -87,9 +94,9 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
                     setattr(mod, n, getattr(ours_tsdf, n))
             if mod.__name__ not in patched:
                 patched.append(mod.__name__)
-        if fuse_color:
+        if wrap:
             _saved.setdefault((fh.__name__, "get_fuser"), fh.get_fuser)
-            fh.get_fuser = _color_get_fuser(_saved[(fh.__name__, "get_fuser")], fh)
+            fh.get_fuser = _color_get_fuser(_saved[(fh.__name__, "get_fuser")], fh, fuse_color, unbounded_fusion)
     if metrics:
         from . import metrics as ours_metrics
         mu = importlib.import_module("utils.metrics_utils")
@@ -129,16 +136,23 @@ def install(verbose: bool = False, losses: bool = False, fusion: bool = False, f
     return patched
 
 
-def _color_get_fuser(original, fh):
-    """``get_fuser`` (tools/fusers_helper.py:188-220) with ``ours`` + ``fuse_color`` -> ``ColorFuser``."""
+def _color_get_fuser(original, fh, color: bool = True, unbounded: bool = False):
+    """``get_fuser`` (tools/fusers_helper.py:188-220) with ``ours`` + ``fuse_color`` -> ``ColorFuser`` (when
+    ``color``), and ``ours`` without a ground-truth mesh -> ``ColorFuser(unbounded=True)`` (when ``unbounded``)."""
     def get_fuser(opts, scan):
-        if getattr(opts, "depth_fuser", None) != "ours" or not getattr(opts, "fuse_color", False):
+        if getattr(opts, "depth_fuser", None) != "ours":
             return original(opts, scan)
-        from .fusers import ColorFuser
+        fuse_color = color and bool(getattr(opts, "fuse_color", False))
         if opts.dataset == "scannet":      # the ground-truth mesh path exactly as get_fuser computes it
             gt_path = fh.ScannetDataset.get_gt_mesh_path(opts.dataset_path, opts.split, scan)
         else:
             gt_path = None
+        from .fusers import ColorFuser
+        if unbounded and gt_path is None:
+            return ColorFuser(gt_path=None, fusion_resolution=opts.fusion_resolution,
+                              max_fusion_depth=opts.fusion_max_depth, fuse_color=fuse_color, unbounded=True)
+        if not fuse_color:
+            return original(opts, scan)
         return ColorFuser(gt_path=gt_path, fusion_resolution=opts.fusion_resolution,
                           max_fusion_depth=opts.fusion_max_depth, fuse_color=True)
     get_fuser.__wrapped__ = original

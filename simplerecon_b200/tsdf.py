@@ -138,33 +138,14 @@ class TSDF:
     def to_mesh(self, scale_to_world: bool = True, export_single_mesh: bool = False):
         """A ``trimesh.Trimesh`` built as the reference builds it (:156).  Needs trimesh; without
         it, use ``extract_mesh`` (tensors) or ``save`` (PLY file)."""
-        try:
-            import trimesh
-        except ImportError as e:
-            raise ImportError("TSDF.to_mesh needs trimesh; TSDF.extract_mesh returns the mesh as tensors and "
-                              "TSDF.save writes a PLY file without it") from e
-        if self.tsdf_colors is not None:     # vertex colours as uint8 rint(255 c) (DESIGN §4.11)
-            verts, faces, norms, colors = self.extract_mesh(scale_to_world=scale_to_world,
-                                                            single_mesh=export_single_mesh, with_colors=True)
-            return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(),
-                                   normals=norms.cpu().numpy(), vertex_colors=colors_to_u8(colors))
-        verts, faces, norms = self.extract_mesh(scale_to_world=scale_to_world, single_mesh=export_single_mesh)
-        return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(), normals=norms.cpu().numpy())
+        return _to_trimesh(self, self.tsdf_colors is not None, scale_to_world, export_single_mesh)
 
     def save(self, savepath, filename, save_mesh: bool = True):
         """Writes the mesh to ``savepath/filename`` with ``.bin`` replaced by ``.ply`` (:159-168):
         binary little-endian PLY, float x/y/z vertices, uchar-counted int faces.  Unlike the
         reference this does not move the volume to the CPU, and it needs no trimesh.  A colour volume
         adds uchar red / green / blue vertex properties."""
-        os.makedirs(savepath, exist_ok=True)
-        if save_mesh:
-            path = os.path.join(savepath, filename).replace(".bin", ".ply")
-            if self.tsdf_colors is not None:
-                verts, faces, _, colors = self.extract_mesh(with_colors=True)
-                write_ply(path, verts.cpu().numpy(), faces.cpu().numpy(), colors_to_u8(colors))
-            else:
-                verts, faces, _ = self.extract_mesh()
-                write_ply(path, verts.cpu().numpy(), faces.cpu().numpy())
+        _save_ply(self, self.tsdf_colors is not None, savepath, filename, save_mesh)
 
     def cuda(self):
         self.tsdf_values = self.tsdf_values.cuda()
@@ -178,6 +159,218 @@ class TSDF:
         self.tsdf_weights = self.tsdf_weights.cpu()
         if self.tsdf_colors is not None:
             self.tsdf_colors = self.tsdf_colors.cpu()
+        return self
+
+
+def _to_trimesh(vol, colored: bool, scale_to_world: bool, export_single_mesh: bool):
+    """``to_mesh`` of a dense or voxel-block volume: its ``extract_mesh`` as a ``trimesh.Trimesh``."""
+    try:
+        import trimesh
+    except ImportError as e:
+        raise ImportError(f"{type(vol).__name__}.to_mesh needs trimesh; extract_mesh returns the mesh as tensors and "
+                          "save writes a PLY file without it") from e
+    if colored:                              # vertex colours as uint8 rint(255 c) (DESIGN §4.11)
+        verts, faces, norms, colors = vol.extract_mesh(scale_to_world=scale_to_world, single_mesh=export_single_mesh,
+                                                       with_colors=True)
+        return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(),
+                               normals=norms.cpu().numpy(), vertex_colors=colors_to_u8(colors))
+    verts, faces, norms = vol.extract_mesh(scale_to_world=scale_to_world, single_mesh=export_single_mesh)
+    return trimesh.Trimesh(vertices=verts.cpu().numpy(), faces=faces.cpu().numpy(), normals=norms.cpu().numpy())
+
+
+def _save_ply(vol, colored: bool, savepath, filename, save_mesh: bool) -> None:
+    """``save`` of a dense or voxel-block volume: its world-space mesh as a binary PLY."""
+    os.makedirs(savepath, exist_ok=True)
+    if save_mesh:
+        path = os.path.join(savepath, filename).replace(".bin", ".ply")
+        if colored:
+            verts, faces, _, colors = vol.extract_mesh(with_colors=True)
+            write_ply(path, verts.cpu().numpy(), faces.cpu().numpy(), colors_to_u8(colors))
+        else:
+            verts, faces, _ = vol.extract_mesh()
+            write_ply(path, verts.cpu().numpy(), faces.cpu().numpy())
+
+
+# the reference fuser's bounds when no ground-truth mesh gives tighter ones (tools/fusers_helper.py:51-60)
+DEFAULT_BOUNDS = {"xmin": -10.0, "xmax": 10.0, "ymin": -10.0, "ymax": 10.0, "zmin": -10.0, "zmax": 10.0}
+
+
+class SparseCapacityError(RuntimeError):
+    """A ``SparseTSDF`` ran out of block or hash capacity; ``needed`` is the ``max_blocks`` to ask for."""
+
+    def __init__(self, message: str, needed: int):
+        super().__init__(message)
+        self.needed = needed
+
+
+class SparseTSDF:
+    """A TSDF volume without bounds (DESIGN §4.16): the dense ``TSDF``'s lattice and arithmetic, stored as
+    8^3-voxel blocks in a GPU hash table, allocated only where some frame can change a voxel.
+
+    Fed the same frames, it reads back bitwise equal to a dense ``TSDF`` on the same lattice (same
+    ``origin`` and ``voxel_size``) that covers every frustum: values, weights and colours at every voxel,
+    and the same mesh.  Memory is ``max_blocks`` blocks allocated up front: 2 KiB per block (values and
+    weights), 8 KiB with ``color=True``, plus 24 bytes of hash table per block.  ``origin`` fixes the
+    lattice; the default is the reference's ±10 m cube's corner, so the lattice is the one the reference
+    fuses into without a ground-truth mesh.
+
+    Running out of capacity neither corrupts memory nor synchronises: ``to_mesh``, ``extract_mesh``,
+    ``save`` and ``to_dense`` raise a ``SparseCapacityError`` naming the ``max_blocks`` needed."""
+
+    BLOCK = 8
+
+    def __init__(self, voxel_size: float, origin=None, max_blocks: int = 1 << 17, color: bool = False,
+                 device="cuda"):
+        self.voxel_size = float(voxel_size)
+        if origin is None:
+            origin = [DEFAULT_BOUNDS["xmin"], DEFAULT_BOUNDS["ymin"], DEFAULT_BOUNDS["zmin"]]
+        self.origin = torch.as_tensor(origin, dtype=torch.float32).detach().cpu().reshape(3).clone()
+        self.max_blocks = int(max_blocks)
+        self.color = bool(color)
+        lib = _native.load()
+        n = lib.srcv_sparse_tsdf_state_bytes(C.byref(self._desc(None)))
+        if n == 0:
+            raise ValueError(f"max_blocks = {self.max_blocks} is outside 1 .. 2^26")
+        self.state = torch.empty(n, dtype=torch.uint8, device=device)
+        _require_cuda(self.state)
+        with torch.cuda.device(self.state.device):
+            _native.check(lib.srcv_sparse_tsdf_reset(C.byref(self._desc()), self._stream()))
+
+    @classmethod
+    def from_bounds(cls, bounds: dict, voxel_size: float, device="cuda", color: bool = False, **kw):
+        """A volume on the lattice ``TSDF.from_bounds(bounds, ...)`` would have (origin = the minimum corner)."""
+        return cls(voxel_size, origin=[bounds["xmin"], bounds["ymin"], bounds["zmin"]], color=color, device=device, **kw)
+
+    def _desc(self, state=False, truncation_voxels: float = 3.0, max_weight: float = 100.0) -> _native.SparseTsdf:
+        d = _native.SparseTsdf()
+        d.state = None if state is None else self.state.data_ptr()
+        d.max_blocks, d.color = self.max_blocks, int(self.color)
+        for i in range(3):
+            d.origin[i] = float(self.origin[i])
+        d.voxel_size, d.truncation_voxels, d.max_weight = self.voxel_size, truncation_voxels, max_weight
+        return d
+
+    def _stream(self):
+        return C.c_void_p(torch.cuda.current_stream(self.state.device).cuda_stream)
+
+    def header(self) -> list[int]:
+        """The state header (``SRCV_SPARSE_HDR_*``): blocks requested, lost inserts, range flags.  Syncs."""
+        return [int(x) for x in self.state[:4 * _native.SPARSE_HDR_WORDS].view(torch.int32).tolist()]
+
+    @property
+    def allocated_blocks(self) -> int:
+        """Blocks allocated so far (a host synchronisation)."""
+        return min(self.header()[_native.SPARSE_HDR_BLOCKS], self.max_blocks)
+
+    def _check_capacity(self, blocks: int | None = None, what: str = "") -> int:
+        hdr = self.header()
+        req, lost, rng = hdr[_native.SPARSE_HDR_BLOCKS], hdr[_native.SPARSE_HDR_LOST], hdr[_native.SPARSE_HDR_RANGE]
+        if rng:
+            raise RuntimeError("SparseTSDF: a frame reached outside the ±2^23-voxel lattice around the origin or had "
+                               "a singular projection; its voxels were not fused")
+        if req > self.max_blocks or lost:
+            needed = max(req, self.max_blocks + 1) if not lost else max(req, self.max_blocks) * 2
+            raise SparseCapacityError(
+                f"SparseTSDF ran out of capacity{what}: it needs max_blocks >= {needed} "
+                f"(it has {self.max_blocks}); the volume is incomplete, rebuild it with a larger max_blocks", needed)
+        return req
+
+    @torch.no_grad()
+    def extract_mesh(self, scale_to_world: bool = True, single_mesh: bool = False, with_colors: bool = False):
+        """``TSDF.extract_mesh`` on the unbounded lattice: the same ``(verts, faces, normals[, colors])``
+        as a dense volume on this lattice covering every frustum, up to the order of vertices and faces
+        (DESIGN §4.16).  Host synchronisations: the capacity checks and the vertex / face counts."""
+        if with_colors and not self.color:
+            raise ValueError("with_colors=True needs a colour volume (SparseTSDF(..., color=True))")
+        lib = _native.load()
+        dev = self.state.device
+        n = self._check_capacity()
+        desc = self._desc()
+        with torch.cuda.device(dev):
+            stream = self._stream()
+            _native.check(lib.srcv_sparse_tsdf_mesh_begin(C.byref(desc), n, stream))
+            try:
+                nmesh = self._check_capacity(what=" for the mesh's boundary blocks")
+                a = _native.SparseMeshArgs()
+                a.blocks = nmesh
+                origin_h = self.origin.half().float()
+                for i in range(3):
+                    a.origin[i] = float(origin_h[i])
+                a.scale_to_world, a.single_mesh = int(bool(scale_to_world)), int(bool(single_mesh))
+                nbytes = lib.srcv_sparse_tsdf_mesh_workspace_bytes(C.byref(a))
+                ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+                counts = torch.empty(2, device=dev, dtype=torch.int64)
+                _native.check(lib.srcv_sparse_tsdf_mesh_count(C.byref(desc), C.byref(a), C.c_void_p(counts.data_ptr()),
+                                                              C.c_void_p(ws.data_ptr()), nbytes, stream))
+                V, F = (int(c) for c in counts.tolist())
+                verts = torch.empty((V, 3), device=dev, dtype=torch.float32)
+                normals = torch.empty((V, 3), device=dev, dtype=torch.float32)
+                faces = torch.empty((F, 3), device=dev, dtype=torch.int32)
+                colors = torch.empty((V, 3), device=dev, dtype=torch.float32) if with_colors else None
+                ptr = lambda t: C.c_void_p(t.data_ptr() if t is not None and t.numel() else 0)
+                _native.check(lib.srcv_sparse_tsdf_mesh_extract(
+                    C.byref(desc), C.byref(a), ptr(verts), ptr(normals), ptr(colors) if with_colors else None,
+                    ptr(faces), V, F, C.c_void_p(ws.data_ptr()), nbytes, stream))
+            finally:
+                _native.check(lib.srcv_sparse_tsdf_mesh_end(C.byref(desc), n, stream))
+        return (verts, faces, normals, colors) if with_colors else (verts, faces, normals)
+
+    def to_mesh(self, scale_to_world: bool = True, export_single_mesh: bool = False):
+        """``TSDF.to_mesh``: a ``trimesh.Trimesh`` (vertex colours on a colour volume)."""
+        self._check_capacity()
+        return _to_trimesh(self, self.color, scale_to_world, export_single_mesh)
+
+    def save(self, savepath, filename, save_mesh: bool = True):
+        """``TSDF.save``: the world-space mesh as a binary PLY at ``savepath/filename`` (``.bin`` -> ``.ply``)."""
+        self._check_capacity()
+        _save_ply(self, self.color, savepath, filename, save_mesh)
+
+    @torch.no_grad()
+    def to_dense(self, bounds: dict) -> TSDF:
+        """The dense ``TSDF`` over ``bounds``, as ``TSDF.from_bounds(bounds, voxel_size)`` lays it out but on this
+        volume's lattice: the box starts at the lattice voxel at or below (xmin, ymin, zmin), and its origin is
+        that voxel's position, origin + i * voxel_size in fp32 (so with ``bounds``' minimum corner on the
+        origin, it is exactly ``from_bounds``' volume).  Voxels outside every allocated block read -1 / 0 / 0."""
+        lib = _native.load()
+        self._check_capacity()
+        dims = tuple(int(np.ceil((bounds[a + "max"] - bounds[a + "min"]) / self.voxel_size / TSDF.VOX_MOD)) * TSDF.VOX_MOD
+                     for a in "xyz")
+        lo = [int(np.floor(np.float64(np.float32(bounds[a + "min"]) - np.float32(self.origin[i]))
+                           / np.float64(np.float32(self.voxel_size)) + 1e-9)) for i, a in enumerate("xyz")]
+        origin = torch.tensor([np.float32(self.origin[i]) + np.float32(lo[i]) * np.float32(self.voxel_size)
+                               for i in range(3)], dtype=torch.float32)
+        dev = self.state.device
+        values = torch.empty(dims, dtype=torch.float16, device=dev)
+        weights = torch.empty(dims, dtype=torch.float16, device=dev)
+        colors = torch.empty((3, *dims), dtype=torch.float32, device=dev) if self.color else None
+        with torch.cuda.device(dev):
+            _native.check(lib.srcv_sparse_tsdf_read_box(
+                C.byref(self._desc()), (C.c_int32 * 3)(*lo), (C.c_int32 * 3)(*dims), C.c_void_p(values.data_ptr()),
+                C.c_void_p(weights.data_ptr()), C.c_void_p(colors.data_ptr()) if colors is not None else None,
+                self._stream()))
+        return TSDF(values, weights, self.voxel_size, origin, colors)
+
+    def _integrate(self, fr, col, truncation_voxels: float, max_weight: float) -> None:
+        lib = _native.load()
+        desc = self._desc(truncation_voxels=truncation_voxels, max_weight=max_weight)
+        dev = self.state.device
+        with torch.cuda.device(dev):
+            n = lib.srcv_sparse_tsdf_workspace_bytes(C.byref(fr))
+            ws = torch.empty(n, device=dev, dtype=torch.uint8)
+            stream = self._stream()
+            if col is not None:
+                _native.check(lib.srcv_sparse_tsdf_integrate_color_f16(C.byref(desc), C.byref(fr), C.byref(col),
+                                                                       C.c_void_p(ws.data_ptr()), n, stream))
+            else:
+                _native.check(lib.srcv_sparse_tsdf_integrate_f16(C.byref(desc), C.byref(fr), C.c_void_p(ws.data_ptr()),
+                                                                 n, stream))
+
+    def cuda(self):
+        self.state = self.state.cuda()
+        return self
+
+    def cpu(self):
+        self.state = self.state.cpu()
         return self
 
 
@@ -230,7 +423,7 @@ def _require_cuda(t: torch.Tensor) -> None:
 class TSDFFuser:
     """Fuses depth maps into a TSDF volume (reference tools/tsdf.py:173-320)."""
 
-    def __init__(self, tsdf: TSDF, min_depth: float = 0.5, max_depth: float = 5.0, use_gpu: bool = True):
+    def __init__(self, tsdf: TSDF | SparseTSDF, min_depth: float = 0.5, max_depth: float = 5.0, use_gpu: bool = True):
         if not use_gpu:
             raise RuntimeError("use_gpu=False: this fuser has no CPU path")
         self.tsdf = tsdf
@@ -258,15 +451,21 @@ class TSDFFuser:
         ``color_b3hw`` (required on a colour volume, refused on a plain one): (B,3,Hc,Wc) images of any
         size, taken to fp32; ``color_normalized=True`` means ImageNet-normalised as the dataloader hands
         them out (undone with ``reverse_imagenet_normalize``'s constants), False means already in [0, 1].
-        The kernel picks each update's colour pixel with PyTorch's ``nearest`` rule (DESIGN §4.11)."""
-        values, weights = self.tsdf.tsdf_values, self.tsdf.tsdf_weights
-        colors = self.tsdf.tsdf_colors
-        if colors is None and color_b3hw is not None:
+        The kernel picks each update's colour pixel with PyTorch's ``nearest`` rule (DESIGN §4.11).
+
+        On a ``SparseTSDF`` the blocks the frames can reach are allocated first, on the device; nothing
+        synchronises with the host (DESIGN §4.16)."""
+        sparse = isinstance(self.tsdf, SparseTSDF)
+        if sparse:
+            colored, ref = self.tsdf.color, self.tsdf.state
+        else:
+            colored, ref = self.tsdf.tsdf_colors is not None, self.tsdf.tsdf_values
+        if not colored and color_b3hw is not None:
             raise ValueError("color_b3hw given for a volume without colour (TSDF.from_bounds(..., color=True))")
-        if colors is not None and color_b3hw is None:
+        if colored and color_b3hw is None:
             raise ValueError("this volume fuses colour: integrate_depth needs color_b3hw")
-        _require_cuda(values)
-        dev = values.device
+        _require_cuda(ref)
+        dev = ref.device
         lib = _native.load()
         B, _, H, W = depth_b1hw.shape
         depth = depth_b1hw.to(dev).half().contiguous()
@@ -275,23 +474,28 @@ class TSDFFuser:
         mask = None
         if depth_mask_b1hw is not None:
             mask = depth_mask_b1hw.to(dev).to(torch.uint8).contiguous()
+        fr = _native.TsdfFrames(depth.data_ptr(), E.data_ptr(), K.data_ptr(),
+                                mask.data_ptr() if mask is not None else None, B, H, W,
+                                float(self.min_depth), float(self.max_depth))
+        col = None
+        if colored:
+            if color_b3hw.dim() != 4 or color_b3hw.shape[0] != B or color_b3hw.shape[1] != 3:
+                raise ValueError(f"color_b3hw must be ({B}, 3, Hc, Wc), got {tuple(color_b3hw.shape)}")
+            image = color_b3hw.to(dev).float().contiguous()
+            mean, std = (IMAGENET_REVERSE_MEAN, IMAGENET_REVERSE_STD) if color_normalized else ((0.0,) * 3, (1.0,) * 3)
+            planes = None if sparse else self.tsdf.tsdf_colors.data_ptr()     # a SparseTSDF keeps them in its state
+            col = _native.TsdfColor(planes, image.data_ptr(), int(image.shape[2]), int(image.shape[3]),
+                                    (C.c_float * 3)(*mean), (C.c_float * 3)(*std))
+        if sparse:
+            self.tsdf._integrate(fr, col, self.truncation_size, self.maxW)
+            return
+        values, weights = self.tsdf.tsdf_values, self.tsdf.tsdf_weights
         vol = _native.TsdfVolume()
         vol.tsdf_values, vol.tsdf_weights = values.data_ptr(), weights.data_ptr()
         vol.X, vol.Y, vol.Z = (int(d) for d in values.shape)
         for i in range(3):
             vol.origin[i] = float(self.tsdf.origin[i])
         vol.voxel_size, vol.truncation_voxels, vol.max_weight = self.voxel_size, self.truncation_size, self.maxW
-        fr = _native.TsdfFrames(depth.data_ptr(), E.data_ptr(), K.data_ptr(),
-                                mask.data_ptr() if mask is not None else None, B, H, W,
-                                float(self.min_depth), float(self.max_depth))
-        col = None
-        if colors is not None:
-            if color_b3hw.dim() != 4 or color_b3hw.shape[0] != B or color_b3hw.shape[1] != 3:
-                raise ValueError(f"color_b3hw must be ({B}, 3, Hc, Wc), got {tuple(color_b3hw.shape)}")
-            image = color_b3hw.to(dev).float().contiguous()
-            mean, std = (IMAGENET_REVERSE_MEAN, IMAGENET_REVERSE_STD) if color_normalized else ((0.0,) * 3, (1.0,) * 3)
-            col = _native.TsdfColor(colors.data_ptr(), image.data_ptr(), int(image.shape[2]), int(image.shape[3]),
-                                    (C.c_float * 3)(*mean), (C.c_float * 3)(*std))
         with torch.cuda.device(dev):
             n = lib.srcv_tsdf_workspace_bytes(C.byref(fr))
             ws = torch.empty(n, device=dev, dtype=torch.uint8)
