@@ -422,6 +422,51 @@ int32_t srcv_sparse_tsdf_mesh_extract(const srcv_sparse_tsdf* volume, const srcv
 int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* volume, const int32_t lo[3], const int32_t dims[3],
                                   void* values, void* weights, void* colors, void* stream);
 
+/* ---- mesh evaluation (DESIGN §4.17) ------------------------------------------------------ *
+ * Scores a predicted surface P against a ground truth G (metres, fp32 coordinates).  With
+ * d(x, S) = min over s in S of |x - s|, evaluated in fp64 from the fp32 coordinates, and threshold tau:
+ *   acc = mean_p d(p, G)   comp = mean_g d(g, P)   chamfer = (acc + comp) / 2
+ *   precision = share of p with d(p, G) < tau   recall = share of g with d(g, P) < tau
+ *   fscore = 2 precision recall / (precision + recall), 0 when both are 0.
+ * srcv_mesh_sample_f32 draws num_samples points (num_samples,3) f32 uniformly by area from the mesh
+ *   (verts (V,3) f32, faces (num_faces,3) int32, DEVICE): sample i takes uniforms u_k = U(seed, i, k),
+ *   k = 0, 1, 2, with U the counter hash of DESIGN §4.17; its triangle is the first whose inclusive area CDF
+ *   exceeds (i + u0) / num_samples * total area; its point is (1 - sqrt u1) a + sqrt u1 (1 - u2) b +
+ *   sqrt u1 u2 c in fp64.  Same inputs and seed: bitwise the same samples.  5 launches.
+ * srcv_nearest_distances_f32: dist (num_queries) f64 out = d(query, points) for queries (num_queries,3)
+ *   and points (num_points,3) f32, DEVICE; exact (four grid levels plus a brute-force queue).  32 launches;
+ *   a level no query reaches exits at once.
+ * srcv_mesh_metrics_f64: from dist_pred (num_queries = |P|) = d(p, G) and dist_gt (num_points = |G|) =
+ *   d(g, P), metrics (8) f64 out: acc, comp, chamfer, precision, recall, fscore, the flag word, 0.
+ *   fp64 sums and int64 counts in a fixed order.  3 launches.
+ * flags: DEVICE uint32 the caller zeroes; the calls OR into it SRCV_MESH_EVAL_BAD_FACE (a face index outside
+ *   [0, V)), _NONFINITE (a non-finite coordinate or area) and _ZERO_AREA (a mesh of zero total area).  Once a
+ *   bit is set the later kernels read nothing out of bounds and write NaN.  stats: optional DEVICE int64[8],
+ *   written by srcv_nearest_distances_f32: per grid level (cell edge h, 8h, 64h, 512h) the target points its
+ *   search evaluated, then per level the queries it left open (the last of these reached the brute force).
+ * Nothing synchronises with the host.  Limits (SRCV_ERR_SHAPE): 1 <= num_points, num_queries, num_samples
+ * <= 2^28 (the workspace is about 48 bytes per target point and 16 per query, ~25 GB at the limit); 1 <= num_faces, V < 2^31.  The workspace is sized by srcv_mesh_eval_workspace_bytes for the same
+ * args, 256-byte aligned.                                                                                   */
+#define SRCV_MESH_EVAL_BAD_FACE 1u
+#define SRCV_MESH_EVAL_NONFINITE 2u
+#define SRCV_MESH_EVAL_ZERO_AREA 4u
+typedef struct srcv_mesh_eval_args {
+  int64_t num_faces;        /* faces of the mesh sampled (0: no sampling)                  */
+  int64_t num_queries;      /* queries of the distances; |P| of the metrics                */
+  int64_t num_points;       /* target points of the distances; |G| of the metrics          */
+  uint32_t* flags;          /* DEVICE, one word                                            */
+  int64_t* stats;           /* DEVICE int64[8] or NULL                                     */
+} srcv_mesh_eval_args;
+size_t srcv_mesh_eval_workspace_bytes(const srcv_mesh_eval_args* args);
+int32_t srcv_mesh_sample_f32(const srcv_mesh_eval_args* args, const float* verts, int32_t V, const int32_t* faces,
+                             int64_t num_samples, uint64_t seed, float* samples, void* workspace,
+                             size_t workspace_bytes, void* stream);
+int32_t srcv_nearest_distances_f32(const srcv_mesh_eval_args* args, const float* queries, const float* points,
+                                   double* dist, void* workspace, size_t workspace_bytes, void* stream);
+int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* args, const double* dist_pred, const double* dist_gt,
+                              double threshold, double* metrics, void* workspace, size_t workspace_bytes,
+                              void* stream);
+
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py
  * :12-97), which pc_fusion.py:158 runs for every frame of a scan against all the others: for each

@@ -26,3 +26,4 @@ from .losses import MSGradientLoss, MVDepthLoss, ScaleInvariantLoss  # noqa: E40
 from .losses import depth_regression_losses  # noqa: E402,F401  (reference experiment_modules/depth_model.py:447-474)
 from .metrics import compute_depth_metrics, compute_depth_metrics_batched, depth_metrics  # noqa: E402,F401  (reference utils/metrics_utils.py)
 from .normals import NormalGenerator, NormalsLoss  # noqa: E402,F401  (reference geometry_utils.py:92-133, losses.py:57-77)
+from .mesh_eval import mesh_metrics, nearest_distances, sample_surface  # noqa: E402,F401  (mesh metrics, DESIGN §4.17)

@@ -119,6 +119,14 @@ class RegLossArgs(C.Structure):
                 ("w", C.c_int32 * 4), ("B", C.c_int32), ("H", C.c_int32), ("W", C.c_int32), ("si_lambda", C.c_double)]
 
 
+class MeshEvalArgs(C.Structure):
+    _fields_ = [("num_faces", C.c_int64), ("num_queries", C.c_int64), ("num_points", C.c_int64), ("flags", _fp),
+                ("stats", _fp)]
+
+
+MESH_EVAL_BAD_FACE, MESH_EVAL_NONFINITE, MESH_EVAL_ZERO_AREA = 1, 2, 4
+
+
 # every symbol include/srcv_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "srcv_abi_version": (C.c_int32, []),
@@ -173,6 +181,11 @@ SYMBOLS = {
     "srcv_sparse_tsdf_mesh_extract": (C.c_int32, [C.POINTER(SparseTsdf), C.POINTER(SparseMeshArgs), _fp, _fp, _fp, _fp,
                                                   C.c_int64, C.c_int64, _fp, C.c_size_t, _fp]),
     "srcv_sparse_tsdf_read_box": (C.c_int32, [C.POINTER(SparseTsdf), C.c_int32 * 3, C.c_int32 * 3, _fp, _fp, _fp, _fp]),
+    "srcv_mesh_eval_workspace_bytes": (C.c_size_t, [C.POINTER(MeshEvalArgs)]),
+    "srcv_mesh_sample_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, C.c_int32, _fp, C.c_int64, C.c_uint64, _fp, _fp,
+                                         C.c_size_t, _fp]),
+    "srcv_nearest_distances_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_mesh_metrics_f64": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, C.c_double, _fp, _fp, C.c_size_t, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

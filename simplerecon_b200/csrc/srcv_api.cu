@@ -704,6 +704,82 @@ int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* v, const int32_t lo[3]
   return SRCV_OK;
 }
 
+static constexpr long long kMeshEvalMaxPoints = 1ll << 28;   // ~25 GB of workspace at the limit
+
+static bool mesh_eval_dims_ok(const srcv_mesh_eval_args* a) {
+  return a->num_faces >= 0 && a->num_faces <= 2147483647ll && a->num_queries >= 0 &&
+         a->num_queries <= kMeshEvalMaxPoints && a->num_points >= 0 && a->num_points <= kMeshEvalMaxPoints;
+}
+
+size_t srcv_mesh_eval_workspace_bytes(const srcv_mesh_eval_args* a) {
+  if (!a || !mesh_eval_dims_ok(a)) return 0;
+  return mesh_eval_workspace_bytes(*a);
+}
+
+static int32_t check_mesh_eval(const srcv_mesh_eval_args* a, void* workspace, size_t workspace_bytes) {
+  if (!a) return fail(SRCV_ERR_NULL, "mesh-evaluation arguments are NULL");
+  if (!a->flags) return fail(SRCV_ERR_NULL, "flags is NULL");
+  if (!mesh_eval_dims_ok(a))
+    return fail(SRCV_ERR_SHAPE, "bad sizes num_faces=%lld num_queries=%lld num_points=%lld (points at most 2^28)",
+                (long long)a->num_faces, (long long)a->num_queries, (long long)a->num_points);
+  if ((reinterpret_cast<uintptr_t>(a->flags) & 3u) != 0 || (reinterpret_cast<uintptr_t>(a->stats) & 7u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "flags / stats misaligned");
+  return check_workspace(workspace, workspace_bytes, mesh_eval_workspace_bytes(*a));
+}
+
+int32_t srcv_mesh_sample_f32(const srcv_mesh_eval_args* a, const float* verts, int32_t V, const int32_t* faces,
+                             int64_t num_samples, uint64_t seed, float* samples, void* workspace, size_t workspace_bytes,
+                             void* stream_) {
+  if (int32_t e = check_mesh_eval(a, workspace, workspace_bytes)) return e;
+  if (!verts || !faces || !samples) return fail(SRCV_ERR_NULL, "verts / faces / samples is NULL");
+  if (a->num_faces < 1 || V < 1 || num_samples < 1 || num_samples > kMeshEvalMaxPoints)
+    return fail(SRCV_ERR_SHAPE, "empty mesh or bad sample count: V=%d F=%lld num_samples=%lld", V,
+                (long long)a->num_faces, (long long)num_samples);
+  if (((reinterpret_cast<uintptr_t>(verts) | reinterpret_cast<uintptr_t>(faces) | reinterpret_cast<uintptr_t>(samples)) &
+       3u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "verts / faces / samples must be 4-byte aligned");
+  g_last_variant.store("mesh_sample_f32");
+  cudaError_t err = launch_mesh_sample(*a, verts, V, faces, num_samples, seed, samples, workspace,
+                                       static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "mesh_sample");
+  return SRCV_OK;
+}
+
+int32_t srcv_nearest_distances_f32(const srcv_mesh_eval_args* a, const float* queries, const float* points,
+                                   double* dist, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_mesh_eval(a, workspace, workspace_bytes)) return e;
+  if (!queries || !points || !dist) return fail(SRCV_ERR_NULL, "queries / points / dist is NULL");
+  if (a->num_queries < 1 || a->num_points < 1)
+    return fail(SRCV_ERR_SHAPE, "empty point set: num_queries=%lld num_points=%lld", (long long)a->num_queries,
+                (long long)a->num_points);
+  if (((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(points)) & 3u) != 0 ||
+      (reinterpret_cast<uintptr_t>(dist) & 7u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "queries / points must be 4-byte and dist 8-byte aligned");
+  g_last_variant.store("nearest_distances_f32");
+  cudaError_t err = launch_nearest_distances(*a, queries, points, dist, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "nearest_distances");
+  return SRCV_OK;
+}
+
+int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* a, const double* dist_pred, const double* dist_gt,
+                              double threshold, double* metrics, void* workspace, size_t workspace_bytes,
+                              void* stream_) {
+  if (int32_t e = check_mesh_eval(a, workspace, workspace_bytes)) return e;
+  if (!dist_pred || !dist_gt || !metrics) return fail(SRCV_ERR_NULL, "dist_pred / dist_gt / metrics is NULL");
+  if (a->num_queries < 1 || a->num_points < 1)
+    return fail(SRCV_ERR_SHAPE, "empty point set: |P|=%lld |G|=%lld", (long long)a->num_queries,
+                (long long)a->num_points);
+  if (!(threshold > 0.0)) return fail(SRCV_ERR_SHAPE, "threshold must be positive");
+  if (((reinterpret_cast<uintptr_t>(dist_pred) | reinterpret_cast<uintptr_t>(dist_gt) |
+        reinterpret_cast<uintptr_t>(metrics)) & 7u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "f64 arrays must be 8-byte aligned");
+  g_last_variant.store("mesh_metrics_f64");
+  cudaError_t err = launch_mesh_metrics(*a, dist_pred, dist_gt, threshold, metrics, workspace,
+                                        static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "mesh_metrics");
+  return SRCV_OK;
+}
+
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {
   if (!s || s->N <= 0) return 0;
   return mvs_workspace_bytes(s->N);

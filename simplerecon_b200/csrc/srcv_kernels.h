@@ -133,6 +133,16 @@ cudaError_t launch_sparse_mesh_extract(const srcv_sparse_tsdf& v, const srcv_spa
                                        float* normals, float* vert_colors, int32_t* faces, void* workspace,
                                        cudaStream_t stream);
 
+// mesh evaluation: surface sampling, exact nearest distances, metrics (csrc/srcv_mesh_eval.cuh, in the srcv_tsdf.cu unit)
+size_t mesh_eval_workspace_bytes(const srcv_mesh_eval_args& a);
+cudaError_t launch_mesh_sample(const srcv_mesh_eval_args& a, const float* verts, int V, const int32_t* faces,
+                               long long num_samples, unsigned long long seed, float* samples, void* workspace,
+                               cudaStream_t stream);
+cudaError_t launch_nearest_distances(const srcv_mesh_eval_args& a, const float* queries, const float* points,
+                                     double* dist, void* workspace, cudaStream_t stream);
+cudaError_t launch_mesh_metrics(const srcv_mesh_eval_args& a, const double* dist_pred, const double* dist_gt,
+                                double threshold, double* metrics, void* workspace, cudaStream_t stream);
+
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);
 cudaError_t launch_mvs_consistency(const srcv_mvs_scan& s, int ref, float z_thresh, int n_consistent,

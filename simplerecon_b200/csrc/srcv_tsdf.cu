@@ -357,3 +357,5 @@ cudaError_t launch_tsdf_integrate(const srcv_tsdf_volume& v, const srcv_tsdf_fra
 // the voxel-block hashed volume (SparseTSDF): integration through tsdf_integrate_column, meshing through
 // srcv_mesh.cuh's kernels
 #include "srcv_tsdf_sparse.cuh"
+// mesh evaluation (sampling, nearest distances, metrics) of the meshes and point clouds this unit produces
+#include "srcv_mesh_eval.cuh"

@@ -29,6 +29,7 @@
 // or a block outside the packable range raises a header flag.  The Python layer checks the header at
 // its next host-visible point.
 #pragma once
+#include "srcv_block_hash.cuh"
 #include "srcv_kernels.h"
 #ifdef SRCV_HOST_EMU
 #include "emu_tc.h"
@@ -40,24 +41,9 @@ namespace srcv {
 
 namespace {
 
-#ifdef SRCV_HOST_EMU
-// tests/emu provides 32-bit atomics only
-inline unsigned long long atomicCAS(unsigned long long* p, unsigned long long cmp, unsigned long long v) {
-  __atomic_compare_exchange_n(p, &cmp, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED);
-  return cmp;
-}
-inline unsigned long long load_key(const unsigned long long* p) { return __atomic_load_n(p, __ATOMIC_RELAXED); }
-#else
-__device__ __forceinline__ unsigned long long load_key(const unsigned long long* p) {
-  return *reinterpret_cast<const volatile unsigned long long*>(p);
-}
-#endif
-
 constexpr int kSpTile = 8;                             // pixels per allocation tile edge
 constexpr int kSpThreads = 256;
 constexpr int kSpMaxCtas = 2112;                       // grid-stride kernels over the pool: 16 CTAs per SM
-constexpr unsigned long long kEmptyKey = ~0ull;
-constexpr int kKeyBias = 1 << 20;                      // block coordinates in [-2^20, 2^20) pack into 21 bits
 
 struct alignas(16) BlockCoord { int x, y, z, pad; };
 
@@ -98,22 +84,6 @@ SparseState carve_sparse(const srcv_sparse_tsdf& v, size_t* bytes = nullptr) {
   s.hmask = (unsigned)(H - 1);
   if (bytes) *bytes = off;
   return s;
-}
-
-__device__ __forceinline__ bool block_in_range(int bx, int by, int bz) {
-  return bx >= -kKeyBias && bx < kKeyBias && by >= -kKeyBias && by < kKeyBias && bz >= -kKeyBias && bz < kKeyBias;
-}
-
-__device__ __forceinline__ unsigned long long block_key(int bx, int by, int bz) {
-  return ((unsigned long long)(unsigned)(bx + kKeyBias) << 42) | ((unsigned long long)(unsigned)(by + kKeyBias) << 21) |
-         (unsigned long long)(unsigned)(bz + kKeyBias);
-}
-
-__device__ __forceinline__ unsigned block_hash(unsigned long long k, unsigned mask) {
-  k ^= k >> 31; k *= 0x7fb5d329728ea185ull;           // a 64-bit finaliser (murmur3 style)
-  k ^= k >> 27; k *= 0x81dadef4bc2dd44dull;
-  k ^= k >> 33;
-  return (unsigned)k & mask;
 }
 
 // pool slot of block (bx,by,bz), -1 if it is not allocated

@@ -1,0 +1,215 @@
+"""Mesh evaluation on the GPU (csrc/srcv_mesh_eval.cuh, DESIGN §4.17): accuracy, completeness, Chamfer distance,
+precision, recall and F-score of a fused mesh or point cloud against the ground truth.
+
+These are the "Mesh Metrics" of the reference README's tables (Acc, Comp, Chamfer, Precision, Recall,
+F-Score).  The reference scores meshes with TransformerFusion's ``eval.py`` (and a point cloud through the
+same code), which needs open3d or trimesh and a CPU KD-tree.  Here every step runs on the GPU: a seeded
+area-uniform surface sampler, an exact nearest-neighbour search (a hashed uniform grid with a brute-force
+queue for far queries) and a fixed-order fp64 reduction.
+
+Parity with TransformerFusion's or NeuralRecon's scripts is not claimed: their code is not part of the
+reference, and they may apply visibility masks or voxel down-sampling, which this module does not.
+
+With P the predicted points, G the ground-truth points (metres) and d(x, S) = min over s in S of |x - s|,
+evaluated in fp64 from the fp32 coordinates:
+
+    acc = mean d(p, G)    comp = mean d(g, P)    chamfer = (acc + comp) / 2
+    precision = share of p with d(p, G) < threshold    recall = share of g with d(g, P) < threshold
+    fscore = 2 precision recall / (precision + recall), 0 when both are 0
+
+Inputs are CUDA tensors, or numpy arrays, which are moved to the current CUDA device.  Coordinates may be
+fp32 or fp64 and are taken to fp32; faces may be int32 or int64.  There is no CPU path: a CPU tensor raises.
+"""
+from __future__ import annotations
+
+import ctypes as C
+
+import numpy as np
+import torch
+
+from . import _native
+
+KEYS = ("acc", "comp", "chamfer", "precision", "recall", "fscore")
+# samples drawn from each side given as a mesh (10^6: a room-sized scene at about one sample per cm^2)
+DEFAULT_NUM_SAMPLES = 1_000_000
+_MAX_POINTS = 1 << 28
+_FLAG_NAMES = ((_native.MESH_EVAL_BAD_FACE, "a face index outside [0, V)"),
+               (_native.MESH_EVAL_NONFINITE, "a non-finite (NaN or inf) coordinate"),
+               (_native.MESH_EVAL_ZERO_AREA, "a mesh of zero total area"))
+
+
+def _require_cuda(t: torch.Tensor) -> None:
+    """The device gate (tests/ patch exactly this to drive the host-emulated library)."""
+    if t.device.type != "cuda":
+        raise RuntimeError("simplerecon_b200 mesh evaluation runs on CUDA (sm_90a) only; there is no CPU fallback")
+
+
+def _default_device() -> torch.device:
+    """Where numpy inputs go: the current CUDA device."""
+    if not torch.cuda.is_available():
+        raise RuntimeError("simplerecon_b200 mesh evaluation needs a CUDA device; there is no CPU fallback")
+    return torch.device("cuda", torch.cuda.current_device())
+
+
+def _lib():
+    return _native.load()
+
+
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+
+
+def _tensor(x, what: str) -> torch.Tensor:
+    if isinstance(x, np.ndarray):
+        x = torch.from_numpy(np.ascontiguousarray(x)).to(_default_device())
+    if not torch.is_tensor(x):
+        raise TypeError(f"{what} must be a torch tensor or a numpy array, got {type(x).__name__}")
+    _require_cuda(x)
+    return x
+
+
+def _coords(x, what: str) -> torch.Tensor:
+    t = _tensor(x, what)
+    if t.dim() != 2 or t.shape[1] != 3:
+        raise ValueError(f"{what} must be (N, 3), got {tuple(t.shape)}")
+    if t.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"{what} must be float32 or float64, got {t.dtype}")
+    if t.shape[0] == 0:
+        raise ValueError(f"{what} is empty")
+    if t.shape[0] > _MAX_POINTS:
+        raise ValueError(f"{what} has {t.shape[0]} points; at most 2^28 are supported")
+    return t.detach().to(torch.float32).contiguous()
+
+
+def _faces(x, num_verts: int) -> torch.Tensor:
+    t = _tensor(x, "faces")
+    if t.dim() != 2 or t.shape[1] != 3:
+        raise ValueError(f"faces must be (F, 3), got {tuple(t.shape)}")
+    if t.dtype not in (torch.int32, torch.int64):
+        raise ValueError(f"faces must be int32 or int64, got {t.dtype}")
+    if t.shape[0] == 0:
+        raise ValueError("the mesh has no faces")
+    if num_verts >= 1 << 31 or t.shape[0] >= 1 << 31:
+        raise ValueError("meshes are limited to 2^31 - 1 vertices and faces")
+    # int64 indices outside int32 stay outside [0, V) (and raise the device flag) instead of wrapping
+    return t.detach().clamp(-1, num_verts).to(torch.int32).contiguous()
+
+
+def _args(flags, num_faces=0, num_queries=0, num_points=0, stats=None) -> _native.MeshEvalArgs:
+    return _native.MeshEvalArgs(num_faces, num_queries, num_points, flags.data_ptr(),
+                                stats.data_ptr() if stats is not None else None)
+
+
+def _workspace(args, dev) -> torch.Tensor:
+    n = _lib().srcv_mesh_eval_workspace_bytes(C.byref(args))
+    if n == 0:
+        raise ValueError("unsupported mesh-evaluation sizes")
+    return torch.empty(n, dtype=torch.uint8, device=dev)
+
+
+def _sample(verts, faces, num_samples: int, seed: int, flags) -> torch.Tensor:
+    dev = verts.device
+    args = _args(flags, num_faces=faces.shape[0])
+    ws = _workspace(args, dev)
+    out = torch.empty(num_samples, 3, dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_mesh_sample_f32(
+            C.byref(args), C.c_void_p(verts.data_ptr()), verts.shape[0], C.c_void_p(faces.data_ptr()), num_samples,
+            seed % (1 << 64), C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+    return out
+
+
+def _distances(queries, points, flags, stats=None) -> torch.Tensor:
+    dev = queries.device
+    if points.device != dev:
+        raise ValueError(f"queries on {dev} and points on {points.device}")
+    args = _args(flags, num_queries=queries.shape[0], num_points=points.shape[0], stats=stats)
+    ws = _workspace(args, dev)
+    out = torch.empty(queries.shape[0], dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_nearest_distances_f32(
+            C.byref(args), C.c_void_p(queries.data_ptr()), C.c_void_p(points.data_ptr()), C.c_void_p(out.data_ptr()),
+            C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+    return out
+
+
+def _check_count(num_samples: int) -> int:
+    n = int(num_samples)
+    if not 1 <= n <= _MAX_POINTS:
+        raise ValueError(f"num_samples must be in 1 .. 2^28, got {num_samples}")
+    return n
+
+
+def sample_surface(verts, faces, num_samples: int, seed: int = 0) -> torch.Tensor:
+    """``num_samples`` points (N, 3) fp32 drawn uniformly by area from the mesh ``(verts (V,3), faces (F,3))``.
+
+    Sample i is stratified: its triangle is the first whose area CDF exceeds (i + u0) / N of the total area, so
+    the samples come out in triangle order; within it the point is (1 - sqrt u1) a + sqrt u1 (1 - u2) b +
+    sqrt u1 u2 c.  u0, u1, u2 come from a counter hash of (seed, i, draw) (DESIGN §4.17): the same inputs and
+    seed give bitwise the same samples.  A face index outside [0, V), a non-finite coordinate or a zero total
+    area makes every sample NaN (``mesh_metrics`` names the condition).  No host synchronisation."""
+    n = _check_count(num_samples)
+    v = _coords(verts, "verts")
+    f = _faces(faces, v.shape[0])
+    if f.device != v.device:
+        raise ValueError(f"verts on {v.device} and faces on {f.device}")
+    flags = torch.zeros(1, dtype=torch.int32, device=v.device)
+    return _sample(v, f, n, int(seed), flags)
+
+
+def nearest_distances(queries, points) -> torch.Tensor:
+    """(Nq,) fp64: the distance from each query to its nearest point of ``points`` (N, 3), evaluated in fp64
+    from the fp32 coordinates, exactly (the same minimum a fp64 KD-tree finds).  A non-finite coordinate makes
+    every distance NaN.  No host synchronisation."""
+    q = _coords(queries, "queries")
+    p = _coords(points, "points")
+    flags = torch.zeros(1, dtype=torch.int32, device=q.device)
+    return _distances(q, p, flags)
+
+
+def _device_of(x, what: str) -> torch.device:
+    probe = x[0] if isinstance(x, (tuple, list)) else x
+    return _default_device() if isinstance(probe, np.ndarray) else _tensor(probe, what).device
+
+
+def _side(x, what: str, num_samples: int, seed: int, flags) -> torch.Tensor:
+    if isinstance(x, (tuple, list)):
+        if len(x) != 2:
+            raise ValueError(f"{what} must be (verts, faces) or an (N, 3) point set")
+        v = _coords(x[0], f"{what} verts")
+        f = _faces(x[1], v.shape[0])
+        return _sample(v, f, num_samples, seed, flags)
+    return _coords(x, f"{what} points")
+
+
+def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_NUM_SAMPLES, seed: int = 0) -> dict:
+    """{acc, comp, chamfer, precision, recall, fscore} (Python floats, in that order) of ``pred`` against ``gt``.
+
+    Each side is a mesh ``(verts, faces)``, replaced by ``num_samples`` area-uniform surface samples
+    (``sample_surface`` with ``seed`` for ``pred`` and ``seed + 1`` for ``gt``; default 10^6 per side), or a
+    point set ``(N, 3)`` used as given.  ``threshold`` is in metres (default 5 cm).  The result is deterministic:
+    the same inputs and seed give bitwise the same metrics.  One host synchronisation, at the end; a face index
+    outside [0, V), a non-finite coordinate or a mesh of zero total area raises ``ValueError``."""
+    if not threshold > 0:
+        raise ValueError(f"threshold must be positive, got {threshold}")
+    n = _check_count(num_samples)
+    flags = torch.zeros(1, dtype=torch.int32, device=_device_of(pred, "pred"))
+    P = _side(pred, "pred", n, int(seed), flags)
+    G = _side(gt, "gt", n, int(seed) + 1, flags)
+    if P.device != G.device:
+        raise ValueError(f"pred on {P.device} and gt on {G.device}")
+    dev = P.device
+    d_pred = _distances(P, G, flags)
+    d_gt = _distances(G, P, flags)
+    args = _args(flags, num_queries=P.shape[0], num_points=G.shape[0])
+    ws = _workspace(args, dev)
+    out = torch.empty(8, dtype=torch.float64, device=dev)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_mesh_metrics_f64(
+            C.byref(args), C.c_void_p(d_pred.data_ptr()), C.c_void_p(d_gt.data_ptr()), float(threshold),
+            C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+    vals = out.tolist()                                   # the one host synchronisation
+    bad = int(vals[6])
+    if bad:
+        raise ValueError("mesh_metrics: the input has " + " and ".join(name for bit, name in _FLAG_NAMES if bad & bit))
+    return dict(zip(KEYS, vals[:6]))

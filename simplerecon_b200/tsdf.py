@@ -409,6 +409,70 @@ def write_ply(path, verts: np.ndarray, faces: np.ndarray, colors: np.ndarray | N
         f.write(rec.tobytes())
 
 
+_PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2",
+              "ushort": "<u2", "uint16": "<u2", "int": "<i4", "int32": "<i4", "uint": "<u4", "uint32": "<u4",
+              "float": "<f4", "float32": "<f4", "double": "<f8", "float64": "<f8"}
+
+
+def read_ply(path):
+    """``(verts (V,3) float32, faces (F,3) int64 or None)`` from a binary little-endian PLY, such as
+    ``write_ply`` writes or ScanNet's ``_vh_clean_2.ply`` (float x, y, z plus uchar RGBA).
+
+    Vertex x / y / z may be float or double; any other scalar vertex property is skipped by its size.  The
+    optional face element is a list of triangles with a uchar count and int or uint indices.  Other formats
+    (ASCII, big-endian) raise ``ValueError``."""
+    with open(path, "rb") as fh:
+        if fh.readline().strip() != b"ply":
+            raise ValueError(f"{path}: not a PLY file")
+        elements, fmt = [], None
+        while True:
+            line = fh.readline()
+            if not line:
+                raise ValueError(f"{path}: the PLY header has no end_header")
+            tok = line.decode("ascii", "replace").split()
+            if not tok or tok[0] in ("comment", "obj_info"):
+                continue
+            if tok[0] == "end_header":
+                break
+            if tok[0] == "format":
+                fmt = tok[1]
+            elif tok[0] == "element":
+                elements.append((tok[1], int(tok[2]), []))
+            elif tok[0] == "property":
+                if not elements:
+                    raise ValueError(f"{path}: a property before any element")
+                elements[-1][2].append(tok[1:])
+        if fmt != "binary_little_endian":
+            raise ValueError(f"{path}: read_ply reads binary little-endian PLY only, this file is {fmt}")
+        data = fh.read()
+    verts, faces, off = None, None, 0
+    for name, count, props in elements:
+        if any(p[0] == "list" for p in props):
+            if name != "face" or len(props) != 1 or props[0][1] not in ("uchar", "uint8") or \
+                    props[0][2] not in ("int", "int32", "uint", "uint32"):
+                raise ValueError(f"{path}: only a face element of one list (uchar count, int or uint indices) is read")
+            rec = np.dtype([("n", "u1"), ("v", _PLY_TYPES[props[0][2]], (3,))])
+            arr = np.frombuffer(data, dtype=rec, count=count, offset=off)
+            if count and not np.all(arr["n"] == 3):
+                raise ValueError(f"{path}: only triangle faces are read")
+            faces = arr["v"].astype(np.int64)
+            off += rec.itemsize * count
+            continue
+        try:
+            rec = np.dtype([(p[1], _PLY_TYPES[p[0]]) for p in props])
+        except KeyError as e:
+            raise ValueError(f"{path}: unknown PLY property type {e.args[0]}") from None
+        if name == "vertex":
+            if not all(a in rec.names for a in "xyz"):
+                raise ValueError(f"{path}: the vertex element has no x, y, z")
+            arr = np.frombuffer(data, dtype=rec, count=count, offset=off)
+            verts = np.stack([arr[a].astype(np.float32) for a in "xyz"], 1)
+        off += rec.itemsize * count
+    if verts is None:
+        raise ValueError(f"{path}: no vertex element")
+    return verts, faces
+
+
 # reverse_imagenet_normalize (reference utils/generic_utils.py:153-159): torchvision's normalize with these
 IMAGENET_REVERSE_MEAN = (-2.11790393, -2.03571429, -1.80444444)
 IMAGENET_REVERSE_STD = (4.36681223, 4.46428571, 4.44444444)
