@@ -138,28 +138,6 @@ __device__ __forceinline__ void sobel(const float v[3][3], float& gx, float& gy)
   gy = 0.125f * ((v[2][0] - v[0][0]) + 2.0f * (v[2][1] - v[0][1]) + (v[2][2] - v[0][2]));
 }
 
-// one CTA sums a level's partials [p0, p1) in a fixed order
-__device__ __forceinline__ void reduce_partials(const double* psum, const long long* pcnt, unsigned p0, unsigned p1,
-                                                double* s_sum, long long* s_cnt) {
-  double sum = 0.0;
-  long long cnt = 0;
-  for (unsigned i = p0 + threadIdx.x; i < p1; i += kThreads) {
-    sum += psum[i];
-    if (pcnt) cnt += pcnt[i];
-  }
-  __syncthreads();   // the previous level's totals have been read
-  s_sum[threadIdx.x] = sum;
-  s_cnt[threadIdx.x] = cnt;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-      s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
-}
-
 // grid L.cta0[4]: CTA c works inside the level l with cta0[l] <= c < cta0[l+1]; per-CTA fp64 sum of
 // |dGx| + |dGy| over the masked pixels and the count of masked COMPONENTS (two per pixel)
 __global__ void __launch_bounds__(kThreads)
@@ -204,14 +182,10 @@ msgrad_loss_kernel(const float* __restrict__ gt, const float* __restrict__ pred,
   }
   s_sum[threadIdx.x] = sum;
   s_cnt[threadIdx.x] = cnt;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-      s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  block_tree<kThreads>([&](int t, int u) {
+    s_sum[t] += s_sum[u];
+    s_cnt[t] += s_cnt[u];
+  });
   if (threadIdx.x == 0) {
     psum[blockIdx.x] = s_sum[0];
     pcnt[blockIdx.x] = s_cnt[0];
@@ -231,7 +205,7 @@ msgrad_finalize_kernel(const double* __restrict__ psum, const long long* __restr
       if (threadIdx.x == 0) counts[l] = 0;
       continue;
     }
-    reduce_partials(psum, pcnt, L.cta0[l], L.cta0[l + 1], s_sum, s_cnt);
+    reduce_partials<kThreads>(psum, pcnt, L.cta0[l], L.cta0[l + 1], s_sum, s_cnt);
     total += s_sum[0] / (double)s_cnt[0];
     if (threadIdx.x == 0) counts[l] = s_cnt[0];
   }
@@ -334,14 +308,10 @@ si_loss_kernel(const float* __restrict__ gt, const float* __restrict__ pred, lon
   }
   s_a[threadIdx.x] = a;
   s_b[threadIdx.x] = q;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) {
-      s_a[threadIdx.x] += s_a[threadIdx.x + o];
-      s_b[threadIdx.x] += s_b[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  block_tree<kThreads>([&](int t, int u) {
+    s_a[t] += s_a[u];
+    s_b[t] += s_b[u];
+  });
   if (threadIdx.x == 0) {
     psum[blockIdx.x] = s_a[0];
     psq[blockIdx.x] = s_b[0];
@@ -354,9 +324,9 @@ si_loss_finalize_kernel(const double* __restrict__ psum, const double* __restric
                         long long n, double lambda, float* __restrict__ loss, SiStats* __restrict__ stats) {
   __shared__ double s_sum[kThreads];
   __shared__ long long s_unused[kThreads];
-  reduce_partials(psum, nullptr, 0, n_partials, s_sum, s_unused);
+  reduce_partials<kThreads>(psum, nullptr, 0, n_partials, s_sum, s_unused);
   const double sum = s_sum[0];
-  reduce_partials(psq, nullptr, 0, n_partials, s_sum, s_unused);
+  reduce_partials<kThreads>(psq, nullptr, 0, n_partials, s_sum, s_unused);
   if (threadIdx.x == 0) {
     const double mean = sum / (double)n, r = sqrt(s_sum[0] / (double)n - lambda * mean * mean);
     *loss = (float)r;
@@ -382,8 +352,6 @@ inline unsigned si_partials(long long n) {
   return n > 0 ? (unsigned)((n + per - 1) / per) : 1u;
 }
 
-inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
-
 }  // namespace
 }  // namespace gradloss_detail
 
@@ -394,8 +362,8 @@ namespace gd = gradloss_detail;
 // (backward scratch)]
 size_t msgrad_workspace_bytes(int B, int H, int W, int num_scales) {
   const gd::Levels L = gd::make_levels(B, H, W, num_scales);
-  return 256 + gd::align256((size_t)L.cta0[kMsGradMaxScales] * (sizeof(double) + sizeof(long long))) +
-         gd::align256(3 * (size_t)L.per_tensor * sizeof(float));
+  return 256 + align256((size_t)L.cta0[kMsGradMaxScales] * (sizeof(double) + sizeof(long long))) +
+         align256(3 * (size_t)L.per_tensor * sizeof(float));
 }
 
 namespace gradloss_detail {
@@ -456,7 +424,7 @@ cudaError_t launch_msgrad_backward(const float* gt, const float* pred, int B, in
 
 // workspace: [mean: double, loss: double, n: int64, padded to 256 B | partial sums of d | partial sums of d^2]
 size_t si_loss_workspace_bytes(long long n) {
-  return 256 + gd::align256((size_t)gd::si_partials(n) * 2 * sizeof(double));
+  return 256 + align256((size_t)gd::si_partials(n) * 2 * sizeof(double));
 }
 
 cudaError_t launch_si_loss_forward(const float* gt, const float* pred, long long n, double lambda, float* loss,

@@ -10,6 +10,7 @@
 
 #include "../../include/srcv_b200.h"
 #include "srcv_common.cuh"
+#include "srcv_reduce.cuh"
 
 // One spelling for a kernel launch, so that the host emulation (tests/emu) can run the same
 // launcher code: a template kernel name with commas goes in parentheses.
@@ -21,6 +22,9 @@
 #endif
 
 namespace srcv {
+
+// the size of a workspace region, rounded up to the 256-byte alignment of every region
+inline size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
 
 // Workspace carve-up (all offsets 256-byte aligned).
 struct Workspace {

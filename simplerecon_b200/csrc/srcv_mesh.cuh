@@ -498,8 +498,6 @@ struct MeshWs {
   size_t bytes;
 };
 
-size_t align256(size_t n) { return (n + 255) & ~(size_t)255; }
-
 // blocks of the voxel passes; the workspace is sized for the scalar path (the most blocks)
 long long mesh_blocks(const srcv_mesh_args& a, int vec) {
   const long long plane = (long long)a.Y * (a.Z / vec);

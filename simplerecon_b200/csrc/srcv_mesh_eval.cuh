@@ -242,12 +242,9 @@ bbox_kernel(const float* __restrict__ pts, long long n, double* __restrict__ par
   if (bad) raise_flag(flags, SRCV_MESH_EVAL_NONFINITE);
   const int t = threadIdx.x;
   for (int k = 0; k < 3; ++k) { s[k][t] = lo[k]; s[3 + k][t] = hi[k]; }
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if (t < o)
-      for (int k = 0; k < 3; ++k) { s[k][t] = fmin(s[k][t], s[k][t + o]); s[3 + k][t] = fmax(s[3 + k][t], s[3 + k][t + o]); }
-    __syncthreads();
-  }
+  block_tree<kThreads>([&](int i, int j) {
+    for (int k = 0; k < 3; ++k) { s[k][i] = fmin(s[k][i], s[k][j]); s[3 + k][i] = fmax(s[3 + k][i], s[3 + k][j]); }
+  });
   if (t < 6) partial[blockIdx.x * 6 + t] = s[t][0];
 }
 
@@ -452,11 +449,7 @@ near_kernel(const float* __restrict__ queries, long long nq, int level, const Gr
   }
   const int t = threadIdx.x;
   s_cand[t] = cand;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if (t < o) s_cand[t] += s_cand[t + o];
-    __syncthreads();
-  }
+  block_tree<kThreads>([&](int i, int j) { s_cand[i] += s_cand[j]; });
   if (t == 0 && s_cand[0] != 0ull) atomic_add_u64(&counters->candidates[level], s_cand[0]);
 }
 
@@ -521,11 +514,7 @@ reduce_kernel(const double* __restrict__ d, long long n, double tau, Partial* __
   }
   s_sum[t] = sum;
   s_cnt[t] = cnt;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if (t < o) { s_sum[t] += s_sum[t + o]; s_cnt[t] += s_cnt[t + o]; }
-    __syncthreads();
-  }
+  block_tree<kThreads>([&](int i, int j) { s_sum[i] += s_sum[j]; s_cnt[i] += s_cnt[j]; });
   if (t == 0) partial[blockIdx.x] = Partial{s_sum[0], s_cnt[0]};
 }
 
@@ -546,11 +535,7 @@ metrics_finalize_kernel(const Partial* __restrict__ pp, int np_, long long n_pre
     for (int j = t; j < m; j += kThreads) { sum += p[j].sum; cnt += p[j].below; }
     s_sum[t] = sum;
     s_cnt[t] = cnt;
-    __syncthreads();
-    for (int o = kThreads / 2; o > 0; o >>= 1) {
-      if (t < o) { s_sum[t] += s_sum[t + o]; s_cnt[t] += s_cnt[t + o]; }
-      __syncthreads();
-    }
+    block_tree<kThreads>([&](int i, int j) { s_sum[i] += s_sum[j]; s_cnt[i] += s_cnt[j]; });
     const double n = (double)(side ? n_gt : n_pred);
     mean[side] = s_sum[0] / n;
     share[side] = (double)s_cnt[0] / n;
@@ -572,8 +557,6 @@ metrics_finalize_kernel(const Partial* __restrict__ pp, int np_, long long n_pre
 
 // ---- workspace ------------------------------------------------------------------------------------------
 
-size_t al256(size_t n) { return (n + 255) & ~(size_t)255; }
-
 long long hash_slots(long long n) {
   long long h = 1024;
   while (h < 2 * n) h <<= 1;
@@ -591,9 +574,9 @@ SampleWs carve_sample(long long F, void* base) {
   SampleWs w{};
   char* p = static_cast<char*>(base);
   size_t off = 0;
-  w.area = reinterpret_cast<double*>(p + off); off += al256(8 * (size_t)F);
-  w.cdf = reinterpret_cast<double*>(p + off);  off += al256(8 * (size_t)F);
-  w.tile = reinterpret_cast<double*>(p + off); off += al256(8 * (size_t)tiles_of(F));
+  w.area = reinterpret_cast<double*>(p + off); off += align256(8 * (size_t)F);
+  w.cdf = reinterpret_cast<double*>(p + off);  off += align256(8 * (size_t)F);
+  w.tile = reinterpret_cast<double*>(p + off); off += align256(8 * (size_t)tiles_of(F));
   w.bytes = off;
   return w;
 }
@@ -625,28 +608,28 @@ GridWs carve_grid(long long nq, long long np, void* base) {
   GridWs w{};
   char* p = static_cast<char*>(base);
   size_t off = 0;
-  w.g = reinterpret_cast<GridParams*>(p + off);             off += al256(sizeof(GridParams) * kLevels);
-  w.counters = reinterpret_cast<GridCounters*>(p + off);    off += al256(sizeof(GridCounters));
-  w.box = reinterpret_cast<double*>(p + off);               off += al256(sizeof(double) * 6 * kBoxCtas);
-  w.tile = reinterpret_cast<int*>(p + off);                 off += al256(4 * (size_t)tiles_of(hash_slots(np)));
+  w.g = reinterpret_cast<GridParams*>(p + off);             off += align256(sizeof(GridParams) * kLevels);
+  w.counters = reinterpret_cast<GridCounters*>(p + off);    off += align256(sizeof(GridCounters));
+  w.box = reinterpret_cast<double*>(p + off);               off += align256(sizeof(double) * 6 * kBoxCtas);
+  w.tile = reinterpret_cast<int*>(p + off);                 off += align256(4 * (size_t)tiles_of(hash_slots(np)));
   for (int l = 0; l < kLevels; ++l) {
     GridLevel& v = w.level[l];
     v.H = hash_slots((np >> (2 * l)) > 0 ? (np >> (2 * l)) : 1);
-    v.keys = reinterpret_cast<unsigned long long*>(p + off);  off += al256(8 * (size_t)v.H);
-    v.cnt = reinterpret_cast<int*>(p + off);                  off += al256(4 * (size_t)v.H);
-    v.start = reinterpret_cast<int*>(p + off);                off += al256(4 * (size_t)(v.H + 1));
-    if (l == 0) { v.pts4 = reinterpret_cast<float4*>(p + off); off += al256(16 * (size_t)np); }
-    else { v.idx = reinterpret_cast<int*>(p + off);           off += al256(4 * (size_t)np); }
+    v.keys = reinterpret_cast<unsigned long long*>(p + off);  off += align256(8 * (size_t)v.H);
+    v.cnt = reinterpret_cast<int*>(p + off);                  off += align256(4 * (size_t)v.H);
+    v.start = reinterpret_cast<int*>(p + off);                off += align256(4 * (size_t)(v.H + 1));
+    if (l == 0) { v.pts4 = reinterpret_cast<float4*>(p + off); off += align256(16 * (size_t)np); }
+    else { v.idx = reinterpret_cast<int*>(p + off);           off += align256(4 * (size_t)np); }
   }
-  w.d2 = reinterpret_cast<unsigned long long*>(p + off);    off += al256(8 * (size_t)nq);
-  w.queue[0] = reinterpret_cast<int*>(p + off);             off += al256(4 * (size_t)nq);
-  w.queue[1] = reinterpret_cast<int*>(p + off);             off += al256(4 * (size_t)nq);
+  w.d2 = reinterpret_cast<unsigned long long*>(p + off);    off += align256(8 * (size_t)nq);
+  w.queue[0] = reinterpret_cast<int*>(p + off);             off += align256(4 * (size_t)nq);
+  w.queue[1] = reinterpret_cast<int*>(p + off);             off += align256(4 * (size_t)nq);
   w.bytes = off;
   return w;
 }
 
 size_t metrics_ws_bytes(long long n_pred, long long n_gt) {
-  return al256(sizeof(Partial) * (size_t)tiles_of(n_pred)) + al256(sizeof(Partial) * (size_t)tiles_of(n_gt));
+  return align256(sizeof(Partial) * (size_t)tiles_of(n_pred)) + align256(sizeof(Partial) * (size_t)tiles_of(n_gt));
 }
 
 unsigned capped(long long ctas, long long cap) {
@@ -740,7 +723,7 @@ cudaError_t launch_mesh_metrics(const srcv_mesh_eval_args& a, const double* dist
   namespace me = mesh_eval_detail;
   const long long tp = me::tiles_of(a.num_queries), tg = me::tiles_of(a.num_points);
   me::Partial* pp = static_cast<me::Partial*>(workspace);
-  me::Partial* pg = reinterpret_cast<me::Partial*>(static_cast<char*>(workspace) + me::al256(sizeof(me::Partial) * tp));
+  me::Partial* pg = reinterpret_cast<me::Partial*>(static_cast<char*>(workspace) + align256(sizeof(me::Partial) * tp));
   SRCV_LAUNCH(me::reduce_kernel, (unsigned)tp, me::kThreads, 0, stream, dist_pred, a.num_queries, threshold, pp);
   SRCV_LAUNCH(me::reduce_kernel, (unsigned)tg, me::kThreads, 0, stream, dist_gt, a.num_points, threshold, pg);
   SRCV_LAUNCH(me::metrics_finalize_kernel, 1, me::kThreads, 0, stream, (const me::Partial*)pp, (int)tp, a.num_queries,

@@ -136,16 +136,12 @@ metrics_kernel(srcv_metrics_args a, Slot* __restrict__ partial, float* __restric
 #pragma unroll
   for (int k = 0; k < kCounts; ++k)
     s_red[kSums + k][t].u = ((k <= kThresh ? cnt_a : cnt_n) >> (4 * (k <= kThresh ? k : k - 1 - kThresh))) & 15u;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {      // fixed-order tree
-    if (t < o) {
+  block_tree<kThreads>([&](int i, int j) {
 #pragma unroll
-      for (int k = 0; k < kSums; ++k) s_red[k][t].d += s_red[k][t + o].d;
+    for (int k = 0; k < kSums; ++k) s_red[k][i].d += s_red[k][j].d;
 #pragma unroll
-      for (int k = kSums; k < kSlots; ++k) s_red[k][t].u += s_red[k][t + o].u;
-    }
-    __syncthreads();
-  }
+    for (int k = kSums; k < kSlots; ++k) s_red[k][i].u += s_red[k][j].u;
+  });
   if (t < kSlots) partial[((size_t)b * gridDim.x + blockIdx.x) * kSlots + t] = s_red[t][0];
 }
 
@@ -168,16 +164,12 @@ metrics_finalize_kernel(srcv_metrics_args a, const Slot* __restrict__ partial, i
   for (int k = 0; k < kSums; ++k) s_red[k][t].d = sum[k];
 #pragma unroll
   for (int k = 0; k < kCounts; ++k) s_red[kSums + k][t].u = cnt[k];
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {
-    if (t < o) {
+  block_tree<kThreads>([&](int i, int j) {
 #pragma unroll
-      for (int k = 0; k < kSums; ++k) s_red[k][t].d += s_red[k][t + o].d;
+    for (int k = 0; k < kSums; ++k) s_red[k][i].d += s_red[k][j].d;
 #pragma unroll
-      for (int k = kSums; k < kSlots; ++k) s_red[k][t].u += s_red[k][t + o].u;
-    }
-    __syncthreads();
-  }
+    for (int k = kSums; k < kSlots; ++k) s_red[k][i].u += s_red[k][j].u;
+  });
   if (t != 0) return;
   const double n = (double)s_red[kSums][0].u;
   float* m = metrics + (size_t)b * 12;
@@ -216,7 +208,7 @@ bool metrics_shape_supported(const srcv_metrics_args& a) {
 
 size_t metrics_workspace_bytes(const srcv_metrics_args& a) {
   namespace md = metrics_detail;
-  return (((size_t)a.B * md::blocks_per_frame(a) * md::kSlots * sizeof(md::Slot)) + 255) & ~(size_t)255;
+  return align256((size_t)a.B * md::blocks_per_frame(a) * md::kSlots * sizeof(md::Slot));
 }
 
 cudaError_t launch_metrics(const srcv_metrics_args& a, float* metrics, long long* valid_counts, float* upsampled,

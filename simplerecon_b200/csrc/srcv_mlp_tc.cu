@@ -685,9 +685,8 @@ bool mlp_tc_supported(const srcv_shape& s, const srcv_mlp_weights& w) {
          (long long)s.H * s.W < (1ll << 26);
 }
 
-static size_t image_bytes_aligned() { return (kImageBytes + 255) & ~(size_t)255; }
 // workspace tail of the tensor-core variant: [weight image | per-frame layer-1 bias (B x 128 floats)]
-size_t mlp_tc_extra_bytes(const srcv_shape& s) { return image_bytes_aligned() + (((size_t)s.B * kN * 4 + 255) & ~(size_t)255); }
+size_t mlp_tc_extra_bytes(const srcv_shape& s) { return align256(kImageBytes) + align256((size_t)s.B * kN * 4); }
 size_t mlp_tc_image_bytes() { return kImageBytes; }
 
 cudaError_t launch_mlp_tc_pack(const srcv_mlp_weights& w, void* image, cudaStream_t stream) {
@@ -708,7 +707,7 @@ cudaError_t launch_mlp_tc(const srcv_shape& s, const float* cur, const Workspace
     image = reinterpret_cast<const uint8_t*>(ws.extra);
   }
   // b1 and the 21 pose measures enter layer 1 as a per-frame bias (views were written by the prep pass)
-  float* frame_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws.extra) + image_bytes_aligned());
+  float* frame_bias = reinterpret_cast<float*>(reinterpret_cast<uint8_t*>(ws.extra) + align256(kImageBytes));
   SRCV_LAUNCH(tc_frame_bias_kernel, s.B, kN, 0, stream, w, ws.views, frame_bias);
   note_launch();
   int dev = 0, sms = 1;

@@ -153,8 +153,8 @@ mvloss_kernel(srcv_mvloss_args a, float2* __restrict__ partial, uint8_t* __restr
   }
 }
 
-// loss = (1/K) sum_k sum_k / count_k, fp64, in a fixed order (thread-strided partial sums, then a
-// shared-memory tree: the same association on every run); inv_count[k] for the backward
+// loss = (1/K) sum_k sum_k / count_k, fp64, in a fixed order (thread-strided partial sums, then
+// block_tree: the same association on every run); inv_count[k] for the backward
 __global__ void __launch_bounds__(kThreads)
 mvloss_finalize_kernel(const float2* __restrict__ partial, int n_partials, int K, float* __restrict__ loss,
                        float* __restrict__ inv_count) {
@@ -169,14 +169,10 @@ mvloss_finalize_kernel(const float2* __restrict__ partial, int n_partials, int K
     }
     s_sum[threadIdx.x] = sum;
     s_cnt[threadIdx.x] = cnt;
-    __syncthreads();
-    for (int o = kThreads / 2; o > 0; o >>= 1) {
-      if ((int)threadIdx.x < o) {
-        s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-        s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
-      }
-      __syncthreads();
-    }
+    block_tree<kThreads>([&](int t, int u) {
+      s_sum[t] += s_sum[u];
+      s_cnt[t] += s_cnt[u];
+    });
     if (threadIdx.x == 0) {
       total += s_sum[0] / s_cnt[0];              // an empty view gives 0/0 = NaN, like nanmean of nothing
       inv_count[k] = s_cnt[0] > 0.0 ? (float)(1.0 / s_cnt[0]) : 0.f;
@@ -194,7 +190,7 @@ int mvloss_max_views() { return kMaxViews; }
 
 // workspace: [inv_count: kMaxViews floats, padded to 256 B | partials: B * ceil(HW/256) * K float2]
 size_t mvloss_workspace_bytes(const srcv_mvloss_args& a) {
-  return 256 + ((partial_count(a) * (size_t)a.K * sizeof(float2) + 255) & ~(size_t)255);
+  return 256 + align256(partial_count(a) * (size_t)a.K * sizeof(float2));
 }
 
 cudaError_t launch_mvloss_forward(const srcv_mvloss_args& a, float* loss, uint8_t* valid, float* sampled,

@@ -289,14 +289,10 @@ normals_loss_kernel(const float* __restrict__ gt, const float* __restrict__ pred
   }
   s_sum[threadIdx.x] = sum;
   s_cnt[threadIdx.x] = cnt;
-  __syncthreads();
-  for (int o = kLossThreads / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-      s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  block_tree<kLossThreads>([&](int t, int u) {
+    s_sum[t] += s_sum[u];
+    s_cnt[t] += s_cnt[u];
+  });
   if (threadIdx.x == 0) {
     psum[blockIdx.x] = s_sum[0];
     pcnt[blockIdx.x] = s_cnt[0];
@@ -309,22 +305,7 @@ normals_loss_finalize_kernel(const double* __restrict__ psum, const long long* _
                              float* __restrict__ loss, long long* __restrict__ count) {
   __shared__ double s_sum[kLossThreads];
   __shared__ long long s_cnt[kLossThreads];
-  double sum = 0.0;
-  long long cnt = 0;
-  for (int i = threadIdx.x; i < n_partials; i += kLossThreads) {
-    sum += psum[i];
-    cnt += pcnt[i];
-  }
-  s_sum[threadIdx.x] = sum;
-  s_cnt[threadIdx.x] = cnt;
-  __syncthreads();
-  for (int o = kLossThreads / 2; o > 0; o >>= 1) {
-    if ((int)threadIdx.x < o) {
-      s_sum[threadIdx.x] += s_sum[threadIdx.x + o];
-      s_cnt[threadIdx.x] += s_cnt[threadIdx.x + o];
-    }
-    __syncthreads();
-  }
+  reduce_partials<kLossThreads>(psum, pcnt, 0, n_partials, s_sum, s_cnt);
   if (threadIdx.x == 0) {
     *loss = (float)(s_sum[0] / (double)s_cnt[0]);
     *count = s_cnt[0];
@@ -366,7 +347,7 @@ namespace nd = normals_detail;
 
 // workspace: g_Gx, g_Gy as (B,6,H,W) fp32
 size_t normals_workspace_bytes(const srcv_normals_args& a) {
-  return ((size_t)a.B * 6 * a.H * a.W * sizeof(float) + 255) & ~(size_t)255;
+  return align256((size_t)a.B * 6 * a.H * a.W * sizeof(float));
 }
 
 cudaError_t launch_normals_forward(const srcv_normals_args& a, float* normals, cudaStream_t stream) {
@@ -390,7 +371,7 @@ cudaError_t launch_normals_backward(const srcv_normals_args& a, const float* gra
 // workspace: [count int64 | loss copy, padded to 256 B | partial sums: double | partial counts: int64]
 size_t normals_loss_workspace_bytes(int B, int H, int W) {
   const size_t n = nd::loss_partials(nd::loss_pixels(B, H, W));
-  return 256 + ((n * (sizeof(double) + sizeof(long long)) + 255) & ~(size_t)255);
+  return 256 + align256(n * (sizeof(double) + sizeof(long long)));
 }
 
 cudaError_t launch_normals_loss_forward(const float* gt, const float* pred, int B, int H, int W, float* loss,

@@ -191,8 +191,6 @@ argmax_kernel(srcv_shape s, const float* __restrict__ cost, const float* __restr
 
 }  // namespace
 
-static inline size_t align256(size_t x) { return (x + 255) & ~(size_t)255; }
-
 Workspace carve_workspace(const srcv_shape& s, void* base, bool want_c4, size_t extra_bytes) {
   Workspace ws{};
   size_t off = 0;

@@ -34,14 +34,10 @@ instnorm_c4_kernel(const float* __restrict__ x, int V, int C, int HW, float eps,
   __shared__ double red[8][kThreads];
 #pragma unroll
   for (int c = 0; c < 4; ++c) { red[c][threadIdx.x] = s[c]; red[4 + c][threadIdx.x] = ss[c]; }
-  __syncthreads();
-  for (int stride = kThreads / 2; stride > 0; stride >>= 1) {
-    if ((int)threadIdx.x < stride) {
+  block_tree<kThreads>([&](int i, int j) {
 #pragma unroll
-      for (int c = 0; c < 8; ++c) red[c][threadIdx.x] += red[c][threadIdx.x + stride];
-    }
-    __syncthreads();
-  }
+    for (int c = 0; c < 8; ++c) red[c][i] += red[c][j];
+  });
   float mean[4], invstd[4];
 #pragma unroll
   for (int c = 0; c < 4; ++c) {

@@ -22,10 +22,9 @@
 // Limits (checked by the C ABI, SRCV_ERR_SHAPE): 1 <= B <= 65535; B H W < 2^30 and B h_i w_i < 2^30 (32-bit
 // element indices); every present scale at least 1 x 1; scale 0 is required and is H x W.
 //
-// Compiled as part of the multi-view loss unit (srcv_mvloss.cu) after srcv_gradloss.cuh, whose fixed-order partial
-// reduction it uses, and srcv_metrics.cuh, whose nearest source index it shares.
+// Compiled as part of the multi-view loss unit (srcv_mvloss.cu) after srcv_metrics.cuh, whose nearest source index
+// it shares.
 #pragma once
-#include "srcv_gradloss.cuh"
 #include "srcv_metrics.cuh"
 
 namespace srcv {
@@ -33,10 +32,7 @@ namespace srcv {
 namespace regloss_detail {
 namespace {
 
-using gradloss_detail::align256;
-using gradloss_detail::kPerThread;
-using gradloss_detail::kThreads;
-using gradloss_detail::reduce_partials;
+constexpr int kThreads = 256, kPerThread = 4;
 
 // the per-CTA partial sums, series-major (series k of CTA c at k * n_cta + c)
 enum { kMs, kAbs, kL1, kD, kD2, kInv, kSums };
@@ -117,16 +113,12 @@ regloss_kernel(const float* __restrict__ gt, const uint8_t* __restrict__ mask, c
   for (int k = 0; k < kSums; ++k) s_sum[k][t] = sum[k];
   s_cnt[kCntN][t] = cn;
   s_cnt[kCntM][t] = cm;
-  __syncthreads();
-  for (int o = kThreads / 2; o > 0; o >>= 1) {   // fixed-order tree
-    if (t < o) {
+  block_tree<kThreads>([&](int i, int j) {
 #pragma unroll
-      for (int k = 0; k < kSums; ++k) s_sum[k][t] += s_sum[k][t + o];
+    for (int k = 0; k < kSums; ++k) s_sum[k][i] += s_sum[k][j];
 #pragma unroll
-      for (int k = 0; k < kCounts; ++k) s_cnt[k][t] += s_cnt[k][t + o];
-    }
-    __syncthreads();
-  }
+    for (int k = 0; k < kCounts; ++k) s_cnt[k][i] += s_cnt[k][j];
+  });
   if (t < kSums) psum[(size_t)t * gridDim.x + blockIdx.x] = s_sum[t][0];
   if (t < kCounts) pcnt[(size_t)t * gridDim.x + blockIdx.x] = s_cnt[t][0];
 }
@@ -141,8 +133,8 @@ regloss_finalize_kernel(const double* __restrict__ psum, const long long* __rest
   long long cnt[kCounts] = {0, 0};
   for (int k = 0; k < kSums; ++k) {
     const bool with_count = k < kCounts;
-    reduce_partials(psum + (size_t)k * n_partials, with_count ? pcnt + (size_t)k * n_partials : nullptr, 0,
-                    n_partials, s_sum, s_cnt);
+    reduce_partials<kThreads>(psum + (size_t)k * n_partials, with_count ? pcnt + (size_t)k * n_partials : nullptr,
+                              0, n_partials, s_sum, s_cnt);
     total[k] = s_sum[0];
     if (with_count) cnt[k] = s_cnt[0];
   }

@@ -65,21 +65,19 @@ size_t sparse_hash_slots(int max_blocks) {
   return h;
 }
 
-size_t align256s(size_t n) { return (n + 255) & ~(size_t)255; }
-
 SparseState carve_sparse(const srcv_sparse_tsdf& v, size_t* bytes = nullptr) {
   SparseState s{};
   char* p = static_cast<char*>(v.state);
   const size_t H = sparse_hash_slots(v.max_blocks), nb = (size_t)v.max_blocks, nv = nb * 512;
   size_t off = 0;
   s.hdr = reinterpret_cast<unsigned*>(p + off);            off += 256;
-  s.keys = reinterpret_cast<unsigned long long*>(p + off); off += align256s(8 * H);
-  s.vals = reinterpret_cast<int*>(p + off);                off += align256s(4 * H);
-  s.coords = reinterpret_cast<BlockCoord*>(p + off);       off += align256s(16 * nb);
-  s.val = reinterpret_cast<__half*>(p + off);              off += align256s(2 * nv);
-  s.w = reinterpret_cast<__half*>(p + off);                off += align256s(2 * nv);
+  s.keys = reinterpret_cast<unsigned long long*>(p + off); off += align256(8 * H);
+  s.vals = reinterpret_cast<int*>(p + off);                off += align256(4 * H);
+  s.coords = reinterpret_cast<BlockCoord*>(p + off);       off += align256(16 * nb);
+  s.val = reinterpret_cast<__half*>(p + off);              off += align256(2 * nv);
+  s.w = reinterpret_cast<__half*>(p + off);                off += align256(2 * nv);
   s.col = v.color ? reinterpret_cast<float*>(p + off) : nullptr;
-  if (v.color) off += align256s(12 * nv);
+  if (v.color) off += align256(12 * nv);
   s.max_blocks = v.max_blocks;
   s.hmask = (unsigned)(H - 1);
   if (bytes) *bytes = off;
@@ -415,7 +413,7 @@ size_t sparse_tsdf_state_bytes(const srcv_sparse_tsdf& v) {
 size_t sparse_tsdf_workspace_bytes(const srcv_tsdf_frames& f) {
   const int nb = f.B < kMaxFrames ? f.B : kMaxFrames;
   const size_t tiles = (size_t)((f.W + kSpTile - 1) / kSpTile) * ((f.H + kSpTile - 1) / kSpTile);
-  return align256s(sizeof(TsdfFrame) * kMaxFrames) + align256s(sizeof(float) * nb * tiles);
+  return align256(sizeof(TsdfFrame) * kMaxFrames) + align256(sizeof(float) * nb * tiles);
 }
 
 cudaError_t launch_sparse_tsdf_reset(const srcv_sparse_tsdf& v, cudaStream_t stream) {
@@ -429,7 +427,7 @@ cudaError_t launch_sparse_tsdf_integrate(const srcv_sparse_tsdf& v, const srcv_t
                                          cudaStream_t stream, const srcv_tsdf_color* color) {
   const SparseState s = carve_sparse(v);
   TsdfFrame* frames = reinterpret_cast<TsdfFrame*>(workspace);
-  float* tile_far = reinterpret_cast<float*>(static_cast<char*>(workspace) + align256s(sizeof(TsdfFrame) * kMaxFrames));
+  float* tile_far = reinterpret_cast<float*>(static_cast<char*>(workspace) + align256(sizeof(TsdfFrame) * kMaxFrames));
   const int tiles_x = (f.W + kSpTile - 1) / kSpTile, tiles_y = (f.H + kSpTile - 1) / kSpTile;
   const float max_depth_h = __half2float(__float2half_rn(f.max_depth));
   const int slabs = (int)ceil(((double)max_depth_h * 1.01 + 0.01) / (8.0 * v.voxel_size));
