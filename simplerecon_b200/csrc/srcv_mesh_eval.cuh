@@ -223,6 +223,7 @@ struct GridParams {
 struct GridCounters {
   unsigned queued[kLevels];                // queries each level leaves open (the last level's go to the brute force)
   unsigned overflow[kLevels];              // non-zero: a cell did not fit the level's table; the level is skipped
+                                           // (never at level 0: see probe_limit)
   unsigned long long candidates[kLevels];  // target points each level's search evaluated
 };
 
@@ -293,15 +294,21 @@ grid_clear_kernel(unsigned long long* __restrict__ keys, int* __restrict__ cnt, 
   }
 }
 
-// Every key sits within kMaxProbe slots of its home slot: an insert that would go farther fails (and the caller
-// disables the level), so a lookup can stop after kMaxProbe slots as well.
+// Every key sits within `probes` slots of its home slot: an insert that would go farther fails (and the caller
+// disables the level), so a lookup can stop after as many slots.  A coarser level caps the probe at kMaxProbe.
+// Level 0 may probe its whole table: it has at least 2N slots for at most N cells, so an insert always finds a
+// free slot and no target point is ever left out of the cell-ordered copy every level and the brute force read.
 constexpr unsigned kMaxProbe = 256;
 
+unsigned probe_limit(long long H, int level) {
+  return level == 0 || H < kMaxProbe ? (unsigned)H : kMaxProbe;
+}
+
 // the table slot of cell (x, y, z), inserting it when `insert`; -1 if absent (or it did not fit)
-__device__ __forceinline__ long long cell_slot(unsigned long long* keys, unsigned hmask, int x, int y, int z, bool insert) {
+__device__ __forceinline__ long long cell_slot(unsigned long long* keys, unsigned hmask, unsigned probes, int x, int y,
+                                               int z, bool insert) {
   const unsigned long long key = block_key(x, y, z);
   unsigned h = block_hash(key, hmask);
-  const unsigned probes = hmask + 1 < kMaxProbe ? hmask + 1 : kMaxProbe;
   for (unsigned i = 0; i < probes; ++i) {
     unsigned long long k = insert ? load_key(&keys[h]) : keys[h];
     if (insert && k == kEmptyKey) {
@@ -320,19 +327,19 @@ __device__ __forceinline__ float4 target(const float* __restrict__ pts, const fl
   return pts4 != nullptr ? pts4[i] : make_float4(pts[3 * i], pts[3 * i + 1], pts[3 * i + 2], 0.0f);
 }
 
-__device__ __forceinline__ long long target_cell(unsigned long long* keys, unsigned hmask, const GridParams& g, float4 p,
-                                                 bool insert) {
-  return cell_slot(keys, hmask, point_cell((double)p.x - g.lo[0], g, 0), point_cell((double)p.y - g.lo[1], g, 1),
+__device__ __forceinline__ long long target_cell(unsigned long long* keys, unsigned hmask, unsigned probes,
+                                                 const GridParams& g, float4 p, bool insert) {
+  return cell_slot(keys, hmask, probes, point_cell((double)p.x - g.lo[0], g, 0), point_cell((double)p.y - g.lo[1], g, 1),
                    point_cell((double)p.z - g.lo[2], g, 2), insert);
 }
 
 __global__ void __launch_bounds__(kThreads)
 grid_count_kernel(const float* __restrict__ pts, const float4* __restrict__ pts4, long long n,
                   const GridParams* __restrict__ gp, unsigned long long* __restrict__ keys, int* __restrict__ cnt,
-                  unsigned hmask, GridCounters* gc, int level, const unsigned* flags) {
+                  unsigned hmask, unsigned probes, GridCounters* gc, int level, const unsigned* flags) {
   const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (i >= n || (read_flags(flags) & kBad) != 0u || level_idle(gc, level)) return;
-  const long long s = target_cell(keys, hmask, *gp, target(pts, pts4, i), true);
+  const long long s = target_cell(keys, hmask, probes, *gp, target(pts, pts4, i), true);
   if (s >= 0) atomicAdd(reinterpret_cast<unsigned*>(&cnt[s]), 1u);
   else atomicOr(reinterpret_cast<int*>(&gc->overflow[level]), 1);
 }
@@ -343,12 +350,12 @@ grid_count_kernel(const float* __restrict__ pts, const float4* __restrict__ pts4
 __global__ void __launch_bounds__(kThreads)
 grid_scatter_kernel(const float* __restrict__ pts, const float4* __restrict__ pts4, long long n,
                     const GridParams* __restrict__ gp, unsigned long long* __restrict__ keys, int* __restrict__ cnt,
-                    const int* __restrict__ start, unsigned hmask, float4* __restrict__ out4, int* __restrict__ out_idx,
-                    const GridCounters* gc, int level, const unsigned* flags) {
+                    const int* __restrict__ start, unsigned hmask, unsigned probes, float4* __restrict__ out4,
+                    int* __restrict__ out_idx, const GridCounters* gc, int level, const unsigned* flags) {
   const long long i = (long long)blockIdx.x * kThreads + threadIdx.x;
   if (i >= n || (read_flags(flags) & kBad) != 0u || level_idle(gc, level)) return;
   const float4 p = target(pts, pts4, i);
-  const long long s = target_cell(keys, hmask, *gp, p, false);
+  const long long s = target_cell(keys, hmask, probes, *gp, p, false);
   if (s < 0) return;
   const int j = start[s] + (int)atomicAdd(reinterpret_cast<unsigned*>(&cnt[s]), 0xffffffffu) - 1;
   if (out4 != nullptr) out4[j] = p;
@@ -376,8 +383,8 @@ __device__ __forceinline__ double face_dist(int c, int k, double r, double h) {
 // Returns whether best is final.
 __device__ __forceinline__ bool shell_search(double qx, double qy, double qz, const GridParams& g,
                                           const unsigned long long* __restrict__ keys, const int* __restrict__ start,
-                                          unsigned hmask, const float4* __restrict__ pts4, const int* __restrict__ idx,
-                                          double& best, unsigned long long& cand) {
+                                          unsigned hmask, unsigned probes, const float4* __restrict__ pts4,
+                                          const int* __restrict__ idx, double& best, unsigned long long& cand) {
   const double rx = qx - g.lo[0], ry = qy - g.lo[1], rz = qz - g.lo[2];
   const double fx = floor(rx * g.inv_h), fy = floor(ry * g.inv_h), fz = floor(rz * g.inv_h);
   const double lo = -(double)(kMaxShell + 1);
@@ -403,7 +410,7 @@ __device__ __forceinline__ bool shell_search(double qx, double qy, double qz, co
           const int z = cz + dz;
           if (z < 0 || z >= g.n[2]) continue;
           if (gxy + axis_gap(z, rz, h, delta) > best) continue;  // the cell's box is farther than best
-          const long long sl = cell_slot(const_cast<unsigned long long*>(keys), hmask, x, y, z, false);
+          const long long sl = cell_slot(const_cast<unsigned long long*>(keys), hmask, probes, x, y, z, false);
           if (sl < 0) continue;
           const int e = start[sl + 1], b = start[sl];
           for (int j = b; j < e; ++j) best = fmin(best, sq_dist(qx, qy, qz, pts4[idx != nullptr ? idx[j] : j]));
@@ -427,7 +434,7 @@ __device__ __forceinline__ bool shell_search(double qx, double qy, double qz, co
 __global__ void __launch_bounds__(kThreads, 1)
 near_kernel(const float* __restrict__ queries, long long nq, int level, const GridParams* __restrict__ gp,
             GridCounters* counters, const unsigned long long* __restrict__ keys, const int* __restrict__ start,
-            unsigned hmask, const float4* __restrict__ pts4, const int* __restrict__ idx,
+            unsigned hmask, unsigned probes, const float4* __restrict__ pts4, const int* __restrict__ idx,
             unsigned long long* __restrict__ d2, const int* __restrict__ queue_in, int* __restrict__ queue_out,
             unsigned* flags) {
   __shared__ unsigned long long s_cand[kThreads];
@@ -442,7 +449,7 @@ near_kernel(const float* __restrict__ queries, long long nq, int level, const Gr
       raise_flag(flags, SRCV_MESH_EVAL_NONFINITE);
     } else {
       const bool settled = counters->overflow[level] == 0u &&
-                           shell_search(qx, qy, qz, *gp, keys, start, hmask, pts4, idx, best, cand);
+                           shell_search(qx, qy, qz, *gp, keys, start, hmask, probes, pts4, idx, best, cand);
       if (!settled) queue_out[atomicAdd(&counters->queued[level], 1u)] = (int)i;
     }
     d2[i] = double_bits(best);
@@ -601,9 +608,11 @@ struct GridWs {
   size_t bytes;
 };
 
-// Level l's table: the next power of two >= 2 N / 4^l slots.  Level 0's holds every cell of N points at load <= 1/2;
-// a coarser level's cells are 8^l times larger, so on a surface they are about 64^l times fewer.  Should a
-// level's cells not fit (points spread through a volume), its inserts fail and the level is skipped.
+// Level l's table: the next power of two >= 2 N / 4^l slots.  Level 0's holds every cell of N points at load <= 1/2
+// and probes as far as it must, so it never overflows (however the cells collide) and its cell-ordered copy holds
+// every target point.  A coarser level's cells are 8^l times larger, so on a surface they are about 64^l times
+// fewer; should they not fit (points spread through a volume) within kMaxProbe slots of home, an insert fails and
+// the level is skipped: its queries go on to the next level, which still reads every point of level 0's copy.
 GridWs carve_grid(long long nq, long long np, void* base) {
   GridWs w{};
   char* p = static_cast<char*>(base);
@@ -690,22 +699,22 @@ cudaError_t launch_nearest_distances(const srcv_mesh_eval_args& a, const float* 
   for (int l = 0; l < me::kLevels; ++l) {        // each level: count, scan, scatter, then the search
     const me::GridLevel& v = w.level[l];
     const me::GridParams* g = w.g + l;
-    const unsigned hmask = (unsigned)(v.H - 1);
+    const unsigned hmask = (unsigned)(v.H - 1), probes = me::probe_limit(v.H, l);
     const float* src = l == 0 ? points : nullptr;           // a coarser level reads level 0's copy
     const float4* src4 = l == 0 ? nullptr : pts4;
     SRCV_LAUNCH(me::grid_clear_kernel, me::capped(v.H / me::kThreads, 16 * sms), me::kThreads, 0, stream, v.keys, v.cnt,
                 v.H, (const me::GridCounters*)w.counters, l);
-    SRCV_LAUNCH(me::grid_count_kernel, pc, me::kThreads, 0, stream, src, src4, np, g, v.keys, v.cnt, hmask, w.counters, l,
-                (const unsigned*)a.flags);
+    SRCV_LAUNCH(me::grid_count_kernel, pc, me::kThreads, 0, stream, src, src4, np, g, v.keys, v.cnt, hmask, probes,
+                w.counters, l, (const unsigned*)a.flags);
     note_launch(2);
     cudaError_t err = cudaMemsetAsync(v.start, 0, sizeof(int), stream);
     if (err != cudaSuccess) return err;
     me::launch_scan<int>(v.cnt, v.H, w.tile, v.start + 1, stream);
     SRCV_LAUNCH(me::grid_scatter_kernel, pc, me::kThreads, 0, stream, src, src4, np, g, v.keys, v.cnt,
-                (const int*)v.start, hmask, l == 0 ? v.pts4 : nullptr, v.idx, (const me::GridCounters*)w.counters, l,
+                (const int*)v.start, hmask, probes, l == 0 ? v.pts4 : nullptr, v.idx, (const me::GridCounters*)w.counters, l,
                 (const unsigned*)a.flags);
     SRCV_LAUNCH(me::near_kernel, qc, me::kThreads, 0, stream, queries, nq, l, g, w.counters,
-                (const unsigned long long*)v.keys, (const int*)v.start, hmask, pts4, (const int*)v.idx, w.d2,
+                (const unsigned long long*)v.keys, (const int*)v.start, hmask, probes, pts4, (const int*)v.idx, w.d2,
                 (const int*)w.queue[(l + 1) & 1], w.queue[l & 1], a.flags);
     note_launch(2);
   }
