@@ -373,7 +373,8 @@ int32_t srcv_mesh_extract_color(const srcv_mesh_args* args, const void* colors, 
  *   max_blocks   pool capacity in blocks, 1 .. 2^26
  * Header words: BLOCKS = blocks requested so far (it keeps counting past max_blocks, so after an overflow
  * it is the capacity needed), LOST = inserts that found the hash table full, RANGE = non-zero if a frame
- * reached outside the +-2^23-voxel lattice or had a singular projection.  The state is valid while
+ * reached outside voxel indices -2^23 + 8 .. 2^23 - 1 (blocks -2^20 + 1 .. 2^20 - 1, so that meshing can
+ * insert the block below each one) or had a singular projection.  The state is valid while
  * BLOCKS <= max_blocks and LOST == RANGE == 0; nothing here synchronises to check it.
  * srcv_sparse_tsdf_reset initialises the state (1 launch).  The integrate calls take the dense calls'
  * frames, workspace sizing rule (srcv_sparse_tsdf_workspace_bytes) and colour descriptor (its `colors`

@@ -37,12 +37,13 @@ def sample_index(xy_b2N: torch.Tensor, H: int, W: int):
 
 def integrate(tsdf_values, tsdf_weights, tsdf_colors, origin, voxel_size, depth_b1hw, cam_T_world_b44, K_b44,
               color_b3hw, depth_mask_b1hw=None, min_depth: float = 0.5, max_depth: float = 5.0,
-              mean=REVERSE_MEAN, std=REVERSE_STD):
-    """In-place update of values / weights (fp16 (X,Y,Z)) and colours (fp32 (3,X,Y,Z))."""
+              mean=REVERSE_MEAN, std=REVERSE_STD, lo=(0, 0, 0)):
+    """In-place update of values / weights (fp16 (X,Y,Z)) and colours (fp32 (3,X,Y,Z)); ``lo`` as in
+    tsdf_oracle.integrate (the volume holds lattice indices lo .. lo + dims - 1)."""
     dims = tuple(tsdf_values.shape)
     B, _, H, W = depth_b1hw.shape
     Hc, Wc = color_b3hw.shape[-2:]
-    coords = T.voxel_coords(origin, dims, voxel_size)
+    coords = T.voxel_coords(origin, dims, voxel_size, lo)
     trunc = T.TRUNCATION_VOXELS * voxel_size
     depth = depth_b1hw.half()
     if depth_mask_b1hw is not None:

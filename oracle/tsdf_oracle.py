@@ -35,10 +35,11 @@ def volume_dims(bounds: dict, voxel_size: float):
                  for a in "xyz")
 
 
-def voxel_coords(origin: torch.Tensor, dims, voxel_size: float) -> torch.Tensor:
+def voxel_coords(origin: torch.Tensor, dims, voxel_size: float, lo=(0, 0, 0)) -> torch.Tensor:
     """(3,X,Y,Z) fp16 world coordinates: origin + index * voxel_size evaluated in fp32, then
-    .half() (tools/tsdf.py:99-110, :92)."""
-    grid = torch.meshgrid([torch.arange(d) for d in dims], indexing="ij")
+    .half() (tools/tsdf.py:99-110, :92).  ``lo`` offsets the indices: the box of lattice indices
+    lo .. lo + dims - 1 of the lattice at ``origin`` (any sign; a SparseTSDF's lattice is unbounded)."""
+    grid = torch.meshgrid([torch.arange(l, l + d) for l, d in zip(lo, dims)], indexing="ij")
     return (origin.float().view(3, 1, 1, 1) + torch.stack(grid, 0) * voxel_size).half()
 
 
@@ -95,11 +96,12 @@ def overflow_voxels(origin: torch.Tensor, dims, voxel_size: float, cam_T_world_b
 
 def integrate(tsdf_values: torch.Tensor, tsdf_weights: torch.Tensor, origin: torch.Tensor, voxel_size: float,
               depth_b1hw: torch.Tensor, cam_T_world_b44: torch.Tensor, K_b44: torch.Tensor,
-              depth_mask_b1hw: torch.Tensor | None = None, min_depth: float = 0.5, max_depth: float = 5.0):
+              depth_mask_b1hw: torch.Tensor | None = None, min_depth: float = 0.5, max_depth: float = 5.0,
+              lo=(0, 0, 0)):
     """In-place update of (tsdf_values, tsdf_weights) (fp16, (X,Y,Z)) with a batch of depth maps.
-    tools/tsdf.py:221-320."""
+    tools/tsdf.py:221-320.  ``lo``: the volume holds lattice indices lo .. lo + dims - 1 (voxel_coords)."""
     dims = tuple(tsdf_values.shape)
-    coords = voxel_coords(origin, dims, voxel_size)
+    coords = voxel_coords(origin, dims, voxel_size, lo)
     trunc = TRUNCATION_VOXELS * voxel_size                                 # :200-202
     depth = depth_b1hw.half()
     if depth_mask_b1hw is not None:                                        # :251-253

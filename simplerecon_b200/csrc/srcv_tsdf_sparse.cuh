@@ -180,6 +180,10 @@ sparse_alloc_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const fl
   const double v0 = ty * kSpTile - my, v1 = min(ty * kSpTile + kSpTile, p.H) + my;
   // world = M^-1 (cam - t) with M, t the fp16 projection the update uses
   const float* P = frames[b].P;
+  // a non-finite entry (an fp16 overflow of K @ E) makes every voxel's pixel or depth non-finite in the update,
+  // so the frame changes no voxel: nothing to allocate (and no corner below can come out NaN)
+  for (int q = 0; q < 12; ++q)
+    if (!(fabsf(P[q]) <= 65504.0f)) return;           // the fp16 maximum: P was rounded to half
   const double a = P[0], bb = P[1], c = P[2], d = P[4], e = P[5], f = P[6], g = P[8], h = P[9], i = P[10];
   const double A = e * i - f * h, B = f * g - d * i, Cc = d * h - e * g;
   const double det = a * A + bb * B + c * Cc;
@@ -204,7 +208,9 @@ sparse_alloc_kernel(TsdfParams p, const TsdfFrame* __restrict__ frames, const fl
   int blo[3], bhi[3];
   for (int r = 0; r < 3; ++r) {
     const double ilo = floor((lo[r] - margin - o[r]) / p.voxel_size), ihi = ceil((hi[r] + margin - o[r]) / p.voxel_size);
-    if (!(ilo > -8.0 * kKeyBias - 8.0 && ihi < 8.0 * kKeyBias + 8.0)) {   // outside the packable lattice
+    // blocks -2^20 + 1 .. 2^20 - 1: one short of the packable range at the low end, so that meshing can insert
+    // the boundary block below every allocated block
+    if (!(ilo >= -8.0 * (kKeyBias - 1) && ihi < 8.0 * kKeyBias)) {
       atomicOr(reinterpret_cast<int*>(&s.hdr[SRCV_SPARSE_HDR_RANGE]), 1);
       return;
     }

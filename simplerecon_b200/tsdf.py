@@ -266,8 +266,8 @@ class SparseTSDF:
         hdr = self.header()
         req, lost, rng = hdr[_native.SPARSE_HDR_BLOCKS], hdr[_native.SPARSE_HDR_LOST], hdr[_native.SPARSE_HDR_RANGE]
         if rng:
-            raise RuntimeError("SparseTSDF: a frame reached outside the ±2^23-voxel lattice around the origin or had "
-                               "a singular projection; its voxels were not fused")
+            raise RuntimeError("SparseTSDF: a frame reached outside voxel indices -2^23 + 8 .. 2^23 - 1 around the "
+                               "origin or had a singular projection; its voxels were not fused")
         if req > self.max_blocks or lost:
             needed = max(req, self.max_blocks + 1) if not lost else max(req, self.max_blocks) * 2
             raise SparseCapacityError(
