@@ -18,7 +18,7 @@ import ctypes as C
 import torch
 from torch import Tensor, nn
 
-from . import _native
+from . import _native, torch_ops
 from .geometry import BackprojectDepth, Project3D
 from .networks import MLP
 
@@ -54,6 +54,16 @@ def _f32c(t: Tensor, name: str, device) -> Tensor:
     if t.data_ptr() % 16 != 0:      # the kernels use 16-byte vector loads
         t = t.clone()
     return t
+
+
+def _plane_table(planes_bdhw: Tensor, D: int) -> Tensor:
+    """The first ``D`` planes of a ``(B,D',H,W)`` plane tensor as the kernels take them: ``(B,D)``,
+    one depth per plane, when each spatial dimension has stride 0 or size 1 (the expanded view
+    ``generate_depth_planes`` returns), else ``(B,D,H,W)``, one depth per pixel."""
+    st, H, W = planes_bdhw.stride(), planes_bdhw.shape[2], planes_bdhw.shape[3]
+    if (st[2] == 0 or H == 1) and (st[3] == 0 or W == 1):
+        return planes_bdhw[:, :D, 0, 0].contiguous()
+    return planes_bdhw[:, :D].contiguous()
 
 
 def _check_backward_supported(kind: str, src_shape, hidden) -> None:
@@ -99,9 +109,10 @@ def instance_norm_to_chunk_planar(x_bvchw: Tensor, eps: float = 1e-5):
 
 
 class _DotVolumeFunction(torch.autograd.Function):
-    """Differentiable wrapper of the dot-product sweep: fused forward, and a backward kernel
-    (``srcv_dot_backward_f32``) for the two feature inputs — what autograd of the reference's
-    grid_sample / mul / sum composite (modules/cost_volume.py:305-333) yields for them.
+    """Differentiable wrapper of the dot-product sweep: fused forward, and the backward of the
+    ``b200cv::dot_backward`` operator (``srcv_dot_backward_f32``) for the two feature inputs —
+    what autograd of the reference's grid_sample / mul / sum composite
+    (modules/cost_volume.py:305-333) yields for them.
     Cameras and plane depths get no gradient.  fp16 / bf16 features (autocast) are upcast."""
 
     @staticmethod
@@ -119,46 +130,23 @@ class _DotVolumeFunction(torch.autograd.Function):
         cost, lowest, planes_ret, _ = mgr._run_fused(
             cur32, src32, E32, None, Ks32, invK32, min_depth,
             max_depth, depth_planes_bdhw, True, allow_grad=True)
-        B, D, H, W = cost.shape
-        st = planes_ret.stride()
-        per_pixel = not ((st[2] == 0 or H == 1) and (st[3] == 0 or W == 1))
-        planes = planes_ret[:, :D].contiguous() if per_pixel else planes_ret[:, :D, 0, 0].contiguous()
+        planes = _plane_table(planes_ret, cost.shape[1])
         ctx.save_for_backward(cur32, src32, E32, Ks32, invK32, planes)
-        ctx.per_pixel = per_pixel
         ctx.in_dtypes = (cur_feats.dtype, src_feats.dtype)
         ctx.mark_non_differentiable(lowest, planes_ret)
         return cost, lowest, planes_ret
 
     @staticmethod
     def backward(ctx, grad_cost, _grad_lowest, _grad_planes):
-        cur, src, E, Ks, invK, planes = ctx.saved_tensors
-        lib = _native.load()
-        dev = cur.device
-        B, K, Cc, H, W = src.shape
-        D = grad_cost.shape[1]
-        shape = _native.Shape(B, K, Cc, H, W, D)
-        # saved tensors are the dense aligned copies the forward made (see forward)
-        cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
-        pl = _native.Planes()
-        pl.mode = _native.PLANES_PER_PIXEL if ctx.per_pixel else _native.PLANES_PER_PLANE
-        pl.planes = planes.data_ptr()
-        pl.min_depth = pl.max_depth = pl.ramp = pl.planes_out = None
-        g = grad_cost.float().contiguous()
-        with torch.cuda.device(dev):
-            gcur = torch.empty_like(cur)
-            gsrc = torch.empty_like(src)
-            n = lib.srcv_dot_backward_workspace_bytes(C.byref(shape))
-            ws = torch.empty(n, device=dev, dtype=torch.uint8)
-            _native.check(lib.srcv_dot_backward_f32(
-                C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), _ptr(g), _ptr(gcur),
-                _ptr(gsrc), _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        gcur, gsrc = torch_ops._dot_backward(grad_cost.float().contiguous(), *ctx.saved_tensors)
         return (None, gcur.to(ctx.in_dtypes[0]), gsrc.to(ctx.in_dtypes[1]), None, None, None, None, None, None)
 
 
 class _MlpVolumeFunction(torch.autograd.Function):
     """Differentiable wrapper of the metadata-MLP sweep: fused forward (wgmma where the
-    shape allows), and ``srcv_mlp_backward_f32`` — a recompute kernel, nothing but the inputs
-    is saved — for the two feature inputs and the six MLP parameters: what autograd of the
+    shape allows), and the backward of the ``b200cv::mlp_backward`` operator (``srcv_mlp_backward_f32``
+    — a recompute kernel, nothing but the inputs is saved) for the two feature inputs and the six MLP
+    parameters, which it computes on fp32 copies and returns in their own dtype: what autograd of the
     reference composite (modules/cost_volume.py:451-736, modules/networks.py:129-147) yields.
     Cameras and plane depths get no gradient.  fp16 / bf16 features (autocast) are upcast."""
 
@@ -173,12 +161,8 @@ class _MlpVolumeFunction(torch.autograd.Function):
         cost, lowest, planes_ret, mask = mgr._run_fused(
             cur32, src32, cams[0], cams[1], cams[2], cams[3], min_depth, max_depth, depth_planes_bdhw,
             return_mask, True, allow_grad=True)
-        B, D, H, W = cost.shape
-        st = planes_ret.stride()
-        per_pixel = not ((st[2] == 0 or H == 1) and (st[3] == 0 or W == 1))
-        planes = planes_ret[:, :D].contiguous() if per_pixel else planes_ret[:, :D, 0, 0].contiguous()
+        planes = _plane_table(planes_ret, cost.shape[1])
         ctx.save_for_backward(cur32, src32, *cams, planes, w1, b1, w2, b2, w3, b3)
-        ctx.per_pixel = per_pixel
         ctx.in_dtypes = (cur_feats.dtype, src_feats.dtype)
         if mask is None:
             mask = torch.empty(0, dtype=torch.bool, device=cost.device)
@@ -187,32 +171,10 @@ class _MlpVolumeFunction(torch.autograd.Function):
 
     @staticmethod
     def backward(ctx, grad_cost, _gl, _gp, _gm):
-        cur, src, E, P, Ks, invK, planes, *wts = ctx.saved_tensors
-        lib = _native.load()
-        dev = cur.device
-        B, K, Cc, H, W = src.shape
-        D = grad_cost.shape[1]
-        shape = _native.Shape(B, K, Cc, H, W, D)
-        cams = _native.Cameras(E.data_ptr(), P.data_ptr(), Ks.data_ptr(), invK.data_ptr())
-        pl = _native.Planes()
-        pl.mode = _native.PLANES_PER_PIXEL if ctx.per_pixel else _native.PLANES_PER_PLANE
-        pl.planes = planes.data_ptr()
-        pl.min_depth = pl.max_depth = pl.ramp = pl.planes_out = None
-        wc = [_f32c(t.detach(), "mlp parameter", dev) for t in wts]
-        w = _native.MlpWeights(*[t.data_ptr() for t in wc], wc[0].shape[0], wc[2].shape[0], None)
-        g = grad_cost.float().contiguous()
-        with torch.cuda.device(dev):
-            gcur, gsrc = torch.empty_like(cur), torch.empty_like(src)
-            gw = [torch.empty_like(t) for t in wc]
-            grads = _native.MlpGrads(*[t.data_ptr() for t in gw])
-            n = lib.srcv_mlp_backward_workspace_bytes(C.byref(shape), C.byref(w))
-            if n == 0:
-                raise NotImplementedError("metadata-MLP backward: at most 208 input features, hidden widths <= 128")
-            ws = torch.empty(n, device=dev, dtype=torch.uint8)
-            _native.check(lib.srcv_mlp_backward_f32(
-                C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), C.byref(w), _ptr(g),
-                _ptr(gcur), _ptr(gsrc), C.byref(grads), _ptr(ws), n,
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        *inputs, w1, b1, w2, b2, w3, b3 = ctx.saved_tensors
+        wts = (w1, b1, w2, b2, w3, b3)
+        gcur, gsrc, *gw = torch_ops._mlp_backward(grad_cost.float().contiguous(), *inputs,
+                                                  *[t.detach().float() for t in wts])
         gw = [a.to(b.dtype) for a, b in zip(gw, wts)]
         return (None, None, gcur.to(ctx.in_dtypes[0]), gsrc.to(ctx.in_dtypes[1]), None, None, None, None,
                 None, None, None, *gw)
@@ -267,10 +229,7 @@ class CostVolumeManager(nn.Module):
         src = _f32c(src_feats, "src_feats", dev).reshape(B, K, Cc, H, W)
         E, Ks = _f32c(src_extrinsics, "src_extrinsics", dev), _f32c(src_Ks, "src_Ks", dev)
         invK = _f32c(cur_invK, "cur_invK", dev)
-        plane = depth_plane_b1hw
-        st = plane.stride()
-        per_pixel = not ((st[2] == 0 or H == 1) and (st[3] == 0 or W == 1))
-        plane_c = plane.contiguous().reshape(B, H * W) if per_pixel else plane[:, 0, 0, 0].contiguous()
+        plane = _plane_table(depth_plane_b1hw, 1)
         shape = _native.Shape(B, K, Cc, H, W, 1)
         cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
         with torch.cuda.device(dev):
@@ -280,7 +239,7 @@ class CostVolumeManager(nn.Module):
             n = lib.srcv_warp_workspace_bytes(C.byref(shape))
             ws = torch.empty(n, device=dev, dtype=torch.uint8)
             _native.check(lib.srcv_warp_features_f32(
-                C.byref(shape), _ptr(src), C.byref(cams), _ptr(plane_c), int(per_pixel), _ptr(warped),
+                C.byref(shape), _ptr(src), C.byref(cams), _ptr(plane), int(plane.dim() == 4), _ptr(warped),
                 _ptr(depths), _ptr(mask), _ptr(ws), n,
                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         world_points_b4N = self.backprojector(depth_plane_b1hw.expand(B, 1, H, W), invK)
@@ -347,9 +306,9 @@ class CostVolumeManager(nn.Module):
             for k in ("src_cam_T_world", "src_world_T_cam", "cur_cam_T_world", "cur_world_T_cam"):
                 t[k] = _f32c(raw_poses[k], k, dev)
         D = self.num_depth_bins
-        pl = _native.Planes()
         keep = []
         if depth_planes_bdhw is None:
+            pl = _native.Planes()
             mn = _f32c(min_depth.to(dev), "min_depth", dev).reshape(-1)
             mx = _f32c(max_depth.to(dev), "max_depth", dev).reshape(-1)
             # one range for the batch ((1,1,1,1), depth_model.py:358-359) or one per frame
@@ -378,15 +337,8 @@ class CostVolumeManager(nn.Module):
                                  f"the manager sweeps {D}")
             if depth_planes_bdhw.dtype != torch.float32 or depth_planes_bdhw.device != dev:
                 raise ValueError("depth_planes_bdhw must be float32 on the features' device")
-            st = depth_planes_bdhw.stride()
-            if (st[2] == 0 or H == 1) and (st[3] == 0 or W == 1):
-                per = depth_planes_bdhw[:, :D, 0, 0].contiguous()
-                pl.mode = _native.PLANES_PER_PLANE
-            else:
-                per = depth_planes_bdhw[:, :D].contiguous()
-                pl.mode = _native.PLANES_PER_PIXEL
-            pl.planes = per.data_ptr()
-            pl.min_depth = pl.max_depth = pl.ramp = pl.planes_out = None
+            per = _plane_table(depth_planes_bdhw, D)
+            pl = torch_ops._planes_struct(per, per.dim() == 4)
             keep.append(per)
             planes_ret = depth_planes_bdhw
         shape = _native.Shape(B, K, Cc, H, W, D,
@@ -609,9 +561,7 @@ class FastFeatureVolumeManager(FeatureVolumeManager):
         src = _f32c(src_feats, "src_feats", dev).reshape(B, K, Cc, H, W)
         E, Ks = _f32c(src_extrinsics, "src_extrinsics", dev), _f32c(src_Ks, "src_Ks", dev)
         invK = _f32c(cur_invK, "cur_invK", dev)
-        st = depth_plane_bdhw.stride()
-        per_pixel = not ((st[2] == 0 or H == 1) and (st[3] == 0 or W == 1))
-        planes = _f32c(depth_plane_bdhw if per_pixel else depth_plane_bdhw[:, :, 0, 0], "depth_plane_bdhw", dev)
+        planes = _f32c(_plane_table(depth_plane_bdhw, D), "depth_plane_bdhw", dev)
         shape = _native.Shape(B, K, Cc, H, W, D)
         cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
         with torch.cuda.device(dev):
@@ -622,7 +572,7 @@ class FastFeatureVolumeManager(FeatureVolumeManager):
             n = lib.srcv_warp_workspace_bytes(C.byref(shape))
             ws = torch.empty(n, device=dev, dtype=torch.uint8)
             _native.check(lib.srcv_warp_features_planes_f32(
-                C.byref(shape), _ptr(src), C.byref(cams), _ptr(planes), int(per_pixel), _ptr(warped),
+                C.byref(shape), _ptr(src), C.byref(cams), _ptr(planes), int(planes.dim() == 4), _ptr(warped),
                 _ptr(depths), _ptr(mask), _ptr(pix), _ptr(ws), n,
                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
         # world points of every plane (:857-873): X = depth * (invK3 @ p), homogeneous

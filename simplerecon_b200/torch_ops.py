@@ -120,9 +120,8 @@ def _(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes):
     return src_feats.new_empty((B, D, H, W)), src_feats.new_empty((B, H, W))
 
 
-@torch.library.custom_op("b200cv::dot_backward", mutates_args=(), device_types="cuda")
-def dot_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor,
-                 src_Ks: Tensor, cur_invK: Tensor, planes: Tensor) -> Tuple[Tensor, Tensor]:
+def _dot_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor,
+                  src_Ks: Tensor, cur_invK: Tensor, planes: Tensor) -> Tuple[Tensor, Tensor]:
     """``(dL/dcur_feats, dL/dsrc_feats)`` given ``dL/dcost``."""
     B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes)
     if tuple(grad_cost.shape) != (B, D, H, W) or grad_cost.dtype != torch.float32:
@@ -142,6 +141,9 @@ def dot_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_ex
             C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), _ptr(g), _ptr(gcur), _ptr(gsrc),
             _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return gcur, gsrc
+
+
+dot_backward = torch.library.custom_op("b200cv::dot_backward", _dot_backward, mutates_args=(), device_types="cuda")
 
 
 @dot_backward.register_fake
@@ -229,11 +231,10 @@ def _(cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, planes,
             src_feats.new_empty((B, H, W), dtype=torch.bool))
 
 
-@torch.library.custom_op("b200cv::mlp_backward", mutates_args=(), device_types="cuda")
-def mlp_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor,
-                 src_poses: Tensor, src_Ks: Tensor, cur_invK: Tensor, planes: Tensor, w1: Tensor, b1: Tensor,
-                 w2: Tensor, b2: Tensor, w3: Tensor, b3: Tensor
-                 ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
+def _mlp_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor,
+                  src_poses: Tensor, src_Ks: Tensor, cur_invK: Tensor, planes: Tensor, w1: Tensor, b1: Tensor,
+                  w2: Tensor, b2: Tensor, w3: Tensor, b3: Tensor
+                  ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
     """``(dL/dcur_feats, dL/dsrc_feats, dL/dw1, dL/db1, dL/dw2, dL/db2, dL/dw3, dL/db3)`` given
     ``dL/dcost`` — a recompute kernel: nothing of the forward is needed but its inputs."""
     B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
@@ -262,6 +263,9 @@ def mlp_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_ex
             C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), C.byref(w), _ptr(g), _ptr(gcur),
             _ptr(gsrc), C.byref(grads), _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return (gcur, gsrc, *gw)
+
+
+mlp_backward = torch.library.custom_op("b200cv::mlp_backward", _mlp_backward, mutates_args=(), device_types="cuda")
 
 
 @mlp_backward.register_fake

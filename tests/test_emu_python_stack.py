@@ -198,6 +198,29 @@ def test_training_with_strided_views_and_half_inputs(emulated, kind):
         assert fhg.grad.dtype == dt and torch.isfinite(fhg.grad.float()).all()
 
 
+def test_training_with_half_mlp_parameters(emulated):
+    """fp16 MLP parameters (``m.mlp.half()``): the backward runs on fp32 copies of them and casts each
+    parameter gradient back to fp16 — the fp32 gradients of the same rounded parameters."""
+    B, K, C, H, W, D = 1, 2, 8, 8, 10, 3
+    t = make_tuple(B, K, H, W, channels=C, seed=25)
+    gcost = torch.randn(B, D, H, W, generator=torch.Generator().manual_seed(26))
+    mh = _hero(K, C, H, W, D).train()
+    mh.mlp.half()
+    m32 = _hero(K, C, H, W, D).train()
+    m32.mlp.load_state_dict({k: v.float() for k, v in mh.mlp.state_dict().items()})
+    feats = []
+    for m in (mh, m32):
+        f = {k: t[k].clone().requires_grad_(True) for k in ("cur_feats", "src_feats")}
+        cost, *_ = m(**{**t, **f})
+        (cost * gcost).sum().backward()
+        feats.append(f)
+    for ph, p32 in zip(mh.mlp.parameters(), m32.mlp.parameters()):
+        assert ph.dtype == ph.grad.dtype == torch.float16 and p32.grad.dtype == torch.float32
+        assert _rel(ph.grad, p32.grad) < 1e-3
+    for k in ("cur_feats", "src_feats"):
+        assert feats[0][k].grad.dtype == torch.float32 and _rel(feats[0][k].grad, feats[1][k].grad) < 1e-5
+
+
 def test_unsupported_training_shape_fails_in_forward(emulated):
     """The dot backward kernel serves C in {8, 16, 32}: a C = 4 training call is refused when the
     graph is built, not at backward() time (ADVICE r1)."""
