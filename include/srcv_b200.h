@@ -468,6 +468,43 @@ int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* args, const double* dis
                               double threshold, double* metrics, void* workspace, size_t workspace_bytes,
                               void* stream);
 
+/* ---- visibility culling for mesh evaluation (DESIGN §4.18) ------------------------------- *
+ * Point p (fp32, metres) is observed by frame f when fusing f's depth map would update a voxel at p.  In fp64
+ * from the fp32 inputs, in this order, with E = cam_T_world[f] (world -> camera) and K = K[f]:
+ *   x = ((E00 px + E01 py) + E02 pz) + E03, likewise y, z;  U = (K00 x + K01 y) + K02 z, likewise V;
+ *   ix = rint(U / z - 0.5), iy = rint(V / z - 0.5), rounding half to even;
+ *   observed <=> 0 < z < max_depth, 0 <= ix < W, 0 <= iy < H, 0 < d < max_depth for d = depths[f, iy, ix],
+ *   and d - z > -margin.
+ * srcv_observation_counts_f32: counts (num_points) int32 in/out += the frames observing each point of points
+ *   (num_points,3) f32, DEVICE.  Integer counts, no other atomics: bitwise deterministic.  Feeding the frames
+ *   in chunks over several calls gives the counts of one call.  1 launch.  stats: optional DEVICE int64[1],
+ *   += the (point, frame) pairs evaluated after the per-tile frustum test (tile_cull).
+ * srcv_compact_observed_f32: kept (num_points,3) f32 out = the points with counts > 0, in input order;
+ *   num_kept DEVICE int64 out = their number.  5 launches; workspace from srcv_mesh_eval_workspace_bytes with
+ *   the same args.
+ * flags (as above): a non-finite point coordinate ORs SRCV_MESH_EVAL_NONFINITE, a non-finite entry of the E rows
+ *   0..2 or the K entries used SRCV_MESH_EVAL_BAD_VIEW; such points and frames observe nothing.
+ * Limits (SRCV_ERR_SHAPE): 1 <= num_points <= 2^28; F, H, W >= 1, H W < 2^31; margin finite and >= 0;
+ * max_depth > 0 (may be +inf).  Nothing synchronises with the host.                                          */
+#define SRCV_MESH_EVAL_BAD_VIEW 8u
+typedef struct srcv_mesh_views {
+  const float* depths;      /* DEVICE (F,H,W) f32, metres                                   */
+  const float* K;           /* DEVICE (F,4,4) f32, or one (4,4) when K_shared               */
+  const float* cam_T_world; /* DEVICE (F,4,4) f32, world -> camera                          */
+  int32_t F, H, W;
+  int32_t K_shared;         /* 1: one K for every frame                                     */
+  double margin;            /* metres, >= 0                                                 */
+  double max_depth;         /* metres, > 0, may be +inf                                     */
+  int32_t tile_cull;        /* 1: skip a frame for a tile of 256 points whose bounding box
+                               lies outside its frustum (the result is the same); 0: test
+                               every frame for every point (for measurement)               */
+} srcv_mesh_views;
+int32_t srcv_observation_counts_f32(const srcv_mesh_eval_args* args, const srcv_mesh_views* views,
+                                    const float* points, int32_t* counts, void* stream);
+int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* args, const float* points, const int32_t* counts,
+                                  float* kept, int64_t* num_kept, void* workspace, size_t workspace_bytes,
+                                  void* stream);
+
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py
  * :12-97), which pc_fusion.py:158 runs for every frame of a scan against all the others: for each

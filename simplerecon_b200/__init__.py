@@ -27,3 +27,4 @@ from .losses import depth_regression_losses  # noqa: E402,F401  (reference exper
 from .metrics import compute_depth_metrics, compute_depth_metrics_batched, depth_metrics  # noqa: E402,F401  (reference utils/metrics_utils.py)
 from .normals import NormalGenerator, NormalsLoss  # noqa: E402,F401  (reference geometry_utils.py:92-133, losses.py:57-77)
 from .mesh_eval import mesh_metrics, nearest_distances, sample_surface  # noqa: E402,F401  (mesh metrics, DESIGN §4.17)
+from .mesh_eval import Views, observation_counts  # noqa: E402,F401  (visibility culling, DESIGN §4.18)

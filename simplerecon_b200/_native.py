@@ -124,7 +124,13 @@ class MeshEvalArgs(C.Structure):
                 ("stats", _fp)]
 
 
-MESH_EVAL_BAD_FACE, MESH_EVAL_NONFINITE, MESH_EVAL_ZERO_AREA = 1, 2, 4
+MESH_EVAL_BAD_FACE, MESH_EVAL_NONFINITE, MESH_EVAL_ZERO_AREA, MESH_EVAL_BAD_VIEW = 1, 2, 4, 8
+
+
+class MeshViews(C.Structure):
+    _fields_ = [("depths", _fp), ("K", _fp), ("cam_T_world", _fp), ("F", C.c_int32), ("H", C.c_int32),
+                ("W", C.c_int32), ("K_shared", C.c_int32), ("margin", C.c_double), ("max_depth", C.c_double),
+                ("tile_cull", C.c_int32)]
 
 
 # every symbol include/srcv_b200.h declares: (restype, argtypes)
@@ -186,6 +192,8 @@ SYMBOLS = {
                                          C.c_size_t, _fp]),
     "srcv_nearest_distances_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_mesh_metrics_f64": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, C.c_double, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_observation_counts_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), C.POINTER(MeshViews), _fp, _fp, _fp]),
+    "srcv_compact_observed_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

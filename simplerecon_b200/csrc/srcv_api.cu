@@ -1,6 +1,7 @@
 // extern "C" surface of libsrcv_b200.so — see include/srcv_b200.h for the contract
 // and the reference interfaces each entry point stands in for.
 #include <atomic>
+#include <cmath>
 #include <cstdarg>
 #include <cstdio>
 #include <cstring>
@@ -711,9 +712,16 @@ static bool mesh_eval_dims_ok(const srcv_mesh_eval_args* a) {
          a->num_queries <= kMeshEvalMaxPoints && a->num_points >= 0 && a->num_points <= kMeshEvalMaxPoints;
 }
 
+// the distance and metric calls, and the compaction of num_points observed points
+static size_t mesh_eval_all_workspace_bytes(const srcv_mesh_eval_args& a) {
+  const size_t n = mesh_eval_workspace_bytes(a);
+  const size_t c = a.num_points > 0 ? observed_compact_workspace_bytes(a.num_points) : 0;
+  return n > c ? n : c;
+}
+
 size_t srcv_mesh_eval_workspace_bytes(const srcv_mesh_eval_args* a) {
   if (!a || !mesh_eval_dims_ok(a)) return 0;
-  return mesh_eval_workspace_bytes(*a);
+  return mesh_eval_all_workspace_bytes(*a);
 }
 
 static int32_t check_mesh_eval(const srcv_mesh_eval_args* a, void* workspace, size_t workspace_bytes) {
@@ -777,6 +785,52 @@ int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* a, const double* dist_p
   cudaError_t err = launch_mesh_metrics(*a, dist_pred, dist_gt, threshold, metrics, workspace,
                                         static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "mesh_metrics");
+  return SRCV_OK;
+}
+
+static int32_t check_observed_points(const srcv_mesh_eval_args* a) {
+  if (!a) return fail(SRCV_ERR_NULL, "mesh-evaluation arguments are NULL");
+  if (!a->flags) return fail(SRCV_ERR_NULL, "flags is NULL");
+  if (a->num_points < 1 || a->num_points > kMeshEvalMaxPoints)
+    return fail(SRCV_ERR_SHAPE, "bad point count num_points=%lld (1 .. 2^28)", (long long)a->num_points);
+  if ((reinterpret_cast<uintptr_t>(a->flags) & 3u) != 0 || (reinterpret_cast<uintptr_t>(a->stats) & 7u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "flags / stats misaligned");
+  return SRCV_OK;
+}
+
+int32_t srcv_observation_counts_f32(const srcv_mesh_eval_args* a, const srcv_mesh_views* v, const float* points,
+                                    int32_t* counts, void* stream_) {
+  if (int32_t e = check_observed_points(a)) return e;
+  if (!v) return fail(SRCV_ERR_NULL, "views is NULL");
+  if (!points || !counts || !v->depths || !v->K || !v->cam_T_world)
+    return fail(SRCV_ERR_NULL, "points / counts / depths / K / cam_T_world is NULL");
+  if (v->F < 1 || v->H < 1 || v->W < 1 || (long long)v->H * v->W >= (1ll << 31))
+    return fail(SRCV_ERR_SHAPE, "bad frames F=%d H=%d W=%d (F, H, W >= 1, H W < 2^31)", v->F, v->H, v->W);
+  if (!(v->margin >= 0.0 && std::isfinite(v->margin)) || !(v->max_depth > 0.0))
+    return fail(SRCV_ERR_SHAPE, "margin must be finite and >= 0, max_depth > 0 (margin=%g max_depth=%g)", v->margin,
+                v->max_depth);
+  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(counts) |
+        reinterpret_cast<uintptr_t>(v->depths) | reinterpret_cast<uintptr_t>(v->K) |
+        reinterpret_cast<uintptr_t>(v->cam_T_world)) & 3u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "points / counts / depths / K / cam_T_world must be 4-byte aligned");
+  g_last_variant.store("observation_counts_f32");
+  cudaError_t err = launch_observation_counts(*a, *v, points, counts, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "observation_counts");
+  return SRCV_OK;
+}
+
+int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* a, const float* points, const int32_t* counts, float* kept,
+                                  int64_t* num_kept, void* workspace, size_t workspace_bytes, void* stream_) {
+  if (int32_t e = check_observed_points(a)) return e;
+  if (!points || !counts || !kept || !num_kept) return fail(SRCV_ERR_NULL, "points / counts / kept / num_kept is NULL");
+  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(counts) | reinterpret_cast<uintptr_t>(kept)) &
+       3u) != 0 || (reinterpret_cast<uintptr_t>(num_kept) & 7u) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "points / counts / kept must be 4-byte and num_kept 8-byte aligned");
+  if (int32_t e = check_workspace(workspace, workspace_bytes, observed_compact_workspace_bytes(a->num_points))) return e;
+  g_last_variant.store("compact_observed_f32");
+  cudaError_t err = launch_compact_observed(*a, points, counts, kept, num_kept, workspace,
+                                            static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "compact_observed");
   return SRCV_OK;
 }
 

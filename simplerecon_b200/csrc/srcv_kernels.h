@@ -146,6 +146,12 @@ cudaError_t launch_nearest_distances(const srcv_mesh_eval_args& a, const float* 
                                      double* dist, void* workspace, cudaStream_t stream);
 cudaError_t launch_mesh_metrics(const srcv_mesh_eval_args& a, const double* dist_pred, const double* dist_gt,
                                 double threshold, double* metrics, void* workspace, cudaStream_t stream);
+// visibility culling of the evaluated points (csrc/srcv_mesh_visibility.cuh, in the srcv_tsdf.cu unit)
+size_t observed_compact_workspace_bytes(long long n);
+cudaError_t launch_observation_counts(const srcv_mesh_eval_args& a, const srcv_mesh_views& v, const float* points,
+                                      int32_t* counts, cudaStream_t stream);
+cudaError_t launch_compact_observed(const srcv_mesh_eval_args& a, const float* points, const int32_t* counts,
+                                    float* kept, int64_t* num_kept, void* workspace, cudaStream_t stream);
 
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);

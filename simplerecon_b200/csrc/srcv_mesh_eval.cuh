@@ -742,3 +742,6 @@ cudaError_t launch_mesh_metrics(const srcv_mesh_eval_args& a, const double* dist
 }
 
 }  // namespace srcv
+
+// visibility culling of the evaluated points (DESIGN §4.18), built on this file's scan and helpers
+#include "srcv_mesh_visibility.cuh"

@@ -8,7 +8,14 @@ area-uniform surface sampler, an exact nearest-neighbour search (a hashed unifor
 queue for far queries) and a fixed-order fp64 reduction.
 
 Parity with TransformerFusion's or NeuralRecon's scripts is not claimed: their code is not part of the
-reference, and they may apply visibility masks or voxel down-sampling, which this module does not.
+reference, and they may apply visibility masks or voxel down-sampling in ways this module does not reproduce.
+Voxel down-sampling is not done here.
+
+Visibility culling (csrc/srcv_mesh_visibility.cuh, DESIGN §4.18): given the depth frames of the scan
+(``Views``), ``observation_counts`` counts the frames that observe each point, and ``mesh_metrics(..., views=)``
+scores only the points of each side that at least one frame observes.  A point is observed by a frame when fusing
+that frame's depth map would update a voxel at the point (the reference fuser's validity rule, with the
+truncation replaced by ``margin``); see ``observation_counts`` for the exact arithmetic.
 
 With P the predicted points, G the ground-truth points (metres) and d(x, S) = min over s in S of |x - s|,
 evaluated in fp64 from the fp32 coordinates:
@@ -23,6 +30,8 @@ fp32 or fp64 and are taken to fp32; faces may be int32 or int64.  There is no CP
 from __future__ import annotations
 
 import ctypes as C
+import math
+from typing import Any, NamedTuple
 
 import numpy as np
 import torch
@@ -35,7 +44,8 @@ DEFAULT_NUM_SAMPLES = 1_000_000
 _MAX_POINTS = 1 << 28
 _FLAG_NAMES = ((_native.MESH_EVAL_BAD_FACE, "a face index outside [0, V)"),
                (_native.MESH_EVAL_NONFINITE, "a non-finite (NaN or inf) coordinate"),
-               (_native.MESH_EVAL_ZERO_AREA, "a mesh of zero total area"))
+               (_native.MESH_EVAL_ZERO_AREA, "a mesh of zero total area"),
+               (_native.MESH_EVAL_BAD_VIEW, "a non-finite entry in a view's K or cam_T_world"))
 
 
 def _require_cuda(t: torch.Tensor) -> None:
@@ -182,14 +192,120 @@ def _side(x, what: str, num_samples: int, seed: int, flags) -> torch.Tensor:
     return _coords(x, f"{what} points")
 
 
-def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_NUM_SAMPLES, seed: int = 0) -> dict:
+class Views(NamedTuple):
+    """The depth frames that decide which points ``mesh_metrics`` scores (DESIGN §4.18).
+
+    ``depths`` (F, 1, H, W) as the reference passes ``depth_b1hw``, or (F, H, W), metres; ``K`` (F, 4, 4)
+    intrinsics at that resolution, or one (4, 4) for every frame; ``cam_T_world`` (F, 4, 4) world -> camera.
+    A point is observed by a frame when 0 < z < ``max_depth``, it projects into the image and the depth d read
+    there satisfies 0 < d < ``max_depth`` and d - z > -``margin`` (metres)."""
+    depths: Any
+    K: Any
+    cam_T_world: Any
+    margin: float = 0.05
+    max_depth: float = math.inf
+
+
+def _frames(x, what: str, shape: tuple, dev) -> torch.Tensor:
+    t = _tensor(x, what)
+    if t.device != dev:
+        raise ValueError(f"{what} on {t.device}, points on {dev}")
+    if not t.is_floating_point():
+        raise ValueError(f"{what} must be floating point, got {t.dtype}")
+    if tuple(t.shape) not in shape:
+        raise ValueError(f"{what} must be {' or '.join(map(str, shape))}, got {tuple(t.shape)}")
+    return t.detach().to(torch.float32).contiguous()
+
+
+def _views(views, dev, tile_cull: bool = True):
+    """(the C struct, the tensors it points into) for ``views`` on device ``dev``."""
+    if not isinstance(views, Views):
+        views = Views(*views)
+    margin, max_depth = float(views.margin), float(views.max_depth)
+    if not (math.isfinite(margin) and margin >= 0.0):
+        raise ValueError(f"margin must be finite and >= 0, got {views.margin}")
+    if not max_depth > 0.0:
+        raise ValueError(f"max_depth must be > 0, got {views.max_depth}")
+    d = _tensor(views.depths, "depths")
+    if d.dim() == 4 and d.shape[1] == 1:
+        d = d[:, 0]
+    if d.dim() != 3 or min(d.shape) == 0:
+        raise ValueError(f"depths must be (F, 1, H, W) or (F, H, W) and not empty, got {tuple(_tensor(views.depths, 'depths').shape)}")
+    F, H, W = d.shape
+    if H * W >= 1 << 31 or F >= 1 << 31:
+        raise ValueError(f"depth frames of {H} x {W} (x {F}) are too large: H W < 2^31")
+    d = _frames(d, "depths", ((F, H, W),), dev)
+    K = _frames(views.K, "K", ((4, 4), (F, 4, 4)), dev)
+    E = _frames(views.cam_T_world, "cam_T_world", ((F, 4, 4),), dev)
+    s = _native.MeshViews(d.data_ptr(), K.data_ptr(), E.data_ptr(), F, H, W, int(K.dim() == 2), margin, max_depth,
+                          int(tile_cull))
+    return s, (d, K, E)
+
+
+def _count(points, vs, counts, flags, stats=None) -> None:
+    dev = points.device
+    args = _args(flags, num_points=points.shape[0], stats=stats)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_observation_counts_f32(C.byref(args), C.byref(vs), C.c_void_p(points.data_ptr()),
+                                                         C.c_void_p(counts.data_ptr()), _stream(dev)))
+
+
+def _compact(points, counts, flags, num_kept) -> torch.Tensor:
+    """The points with count > 0 in input order, at the head of an (N, 3) buffer; their number goes to num_kept."""
+    dev = points.device
+    args = _args(flags, num_points=points.shape[0])
+    ws = _workspace(args, dev)
+    out = torch.empty_like(points)
+    with torch.cuda.device(dev):
+        _native.check(_lib().srcv_compact_observed_f32(
+            C.byref(args), C.c_void_p(points.data_ptr()), C.c_void_p(counts.data_ptr()), C.c_void_p(out.data_ptr()),
+            C.c_void_p(num_kept.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
+    return out
+
+
+def _observation_counts(points, depths, K, cam_T_world, margin=0.05, max_depth=math.inf, counts=None,
+                        tile_cull: bool = True, stats=None) -> torch.Tensor:
+    p = _coords(points, "points")
+    vs, keep = _views(Views(depths, K, cam_T_world, margin, max_depth), p.device, tile_cull)
+    if counts is None:
+        counts = torch.zeros(p.shape[0], dtype=torch.int32, device=p.device)
+    elif not (torch.is_tensor(counts) and counts.dtype == torch.int32 and tuple(counts.shape) == (p.shape[0],)
+              and counts.device == p.device and counts.is_contiguous()):
+        raise ValueError(f"counts must be a contiguous int32 ({p.shape[0]},) tensor on {p.device}")
+    flags = torch.zeros(1, dtype=torch.int32, device=p.device)
+    _count(p, vs, counts, flags, stats)
+    return counts
+
+
+def observation_counts(points, depths, K, cam_T_world, margin: float = 0.05, max_depth: float = math.inf,
+                       counts=None) -> torch.Tensor:
+    """(N,) int32 on the device: how many of the F depth frames observe each point of ``points`` (N, 3).
+
+    ``depths`` (F, 1, H, W) or (F, H, W) metres, ``K`` (F, 4, 4) or one (4, 4), ``cam_T_world`` (F, 4, 4) world ->
+    camera, as ``Views`` describes.  Evaluated in fp64 from the fp32 inputs, in this order: x = ((E00 px + E01 py)
+    + E02 pz) + E03 (likewise y, z), U = (K00 x + K01 y) + K02 z (likewise V), ix = rint(U / z - 0.5) and
+    iy = rint(V / z - 0.5) rounding half to even (``grid_sample(mode="nearest")``); the point is observed when
+    0 < z < max_depth, 0 <= ix < W, 0 <= iy < H, and d = depths[f, iy, ix] has 0 < d < max_depth and
+    d - z > -margin.  A point with a non-finite coordinate, and a frame with a non-finite K or cam_T_world entry,
+    observe nothing (``mesh_metrics`` raises for them).  With ``counts`` (int32 (N,) on the same device) the
+    counts are added into it in place and it is returned, so frames can be fed in chunks or batch by batch.
+    Bitwise deterministic; no host synchronisation."""
+    return _observation_counts(points, depths, K, cam_T_world, margin, max_depth, counts)
+
+
+def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_NUM_SAMPLES, seed: int = 0,
+                 views: Views | None = None) -> dict:
     """{acc, comp, chamfer, precision, recall, fscore} (Python floats, in that order) of ``pred`` against ``gt``.
 
     Each side is a mesh ``(verts, faces)``, replaced by ``num_samples`` area-uniform surface samples
     (``sample_surface`` with ``seed`` for ``pred`` and ``seed + 1`` for ``gt``; default 10^6 per side), or a
     point set ``(N, 3)`` used as given.  ``threshold`` is in metres (default 5 cm).  The result is deterministic:
     the same inputs and seed give bitwise the same metrics.  One host synchronisation, at the end; a face index
-    outside [0, V), a non-finite coordinate or a mesh of zero total area raises ``ValueError``."""
+    outside [0, V), a non-finite coordinate or a mesh of zero total area raises ``ValueError``.
+
+    With ``views`` (``Views``), each side's points that no frame observes (``observation_counts`` == 0) are
+    dropped before the distances; the call then synchronises twice, and a side left with no point, or a view with
+    a non-finite K or cam_T_world entry, raises ``ValueError``."""
     if not threshold > 0:
         raise ValueError(f"threshold must be positive, got {threshold}")
     n = _check_count(num_samples)
@@ -199,6 +315,20 @@ def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_N
     if P.device != G.device:
         raise ValueError(f"pred on {P.device} and gt on {G.device}")
     dev = P.device
+    if views is not None:
+        vs, keep = _views(views, dev)
+        num_kept = torch.zeros(2, dtype=torch.int64, device=dev)
+        sides = []
+        for k, X in enumerate((P, G)):
+            counts = torch.zeros(X.shape[0], dtype=torch.int32, device=dev)
+            _count(X, vs, counts, flags)
+            sides.append(_compact(X, counts, flags, num_kept[k:k + 1]))
+        n_pred, n_gt, bad = torch.cat([num_kept, flags.to(torch.int64)]).tolist()   # the extra host synchronisation
+        _raise_flags(bad)
+        for name, m in (("pred", n_pred), ("gt", n_gt)):
+            if m == 0:
+                raise ValueError(f"mesh_metrics: no point of {name} is observed by the views")
+        P, G = sides[0][:n_pred], sides[1][:n_gt]
     d_pred = _distances(P, G, flags)
     d_gt = _distances(G, P, flags)
     args = _args(flags, num_queries=P.shape[0], num_points=G.shape[0])
@@ -209,7 +339,10 @@ def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_N
             C.byref(args), C.c_void_p(d_pred.data_ptr()), C.c_void_p(d_gt.data_ptr()), float(threshold),
             C.c_void_p(out.data_ptr()), C.c_void_p(ws.data_ptr()), ws.numel(), _stream(dev)))
     vals = out.tolist()                                   # the one host synchronisation
-    bad = int(vals[6])
+    _raise_flags(int(vals[6]))
+    return dict(zip(KEYS, vals[:6]))
+
+
+def _raise_flags(bad: int) -> None:
     if bad:
         raise ValueError("mesh_metrics: the input has " + " and ".join(name for bit, name in _FLAG_NAMES if bad & bit))
-    return dict(zip(KEYS, vals[:6]))
