@@ -21,6 +21,7 @@ from torch import Tensor, nn
 from . import _native, torch_ops
 from .geometry import BackprojectDepth, Project3D
 from .networks import MLP
+from .torch_ops import _ptr
 
 
 def _require_cuda(dev) -> None:
@@ -31,10 +32,6 @@ def _require_cuda(dev) -> None:
         raise RuntimeError(
             "simplerecon_b200 cost volumes run on CUDA (sm_90a) only; got tensors on "
             f"{dev}.  There is no CPU fallback.")
-
-
-def _ptr(t: Tensor | None):
-    return C.c_void_p(t.data_ptr()) if t is not None else C.c_void_p(0)
 
 
 def _f32c(t: Tensor, name: str, device) -> Tensor:
@@ -221,29 +218,41 @@ class CostVolumeManager(nn.Module):
         This is the materialising form the fused sweeps avoid; it is kept because the
         reference exposes it.  ``uv_scale`` is accepted and unused (the kernel works in
         pixel coordinates)."""
+        B, K, Cc = batch_size, num_src_frames, num_feat_channels
+        H, W = self.matching_height, self.matching_width
+        warped, depths, mask, _, invK = self._warp_planes(src_feats, src_extrinsics, src_Ks, cur_invK,
+                                                          depth_plane_b1hw, 1, B, K, Cc, want_pix=False)
+        world_points_b4N = self.backprojector(depth_plane_b1hw.expand(B, 1, H, W), invK)
+        return (world_points_b4N.repeat_interleave(K, dim=0), depths.reshape(B, K, H, W),
+                warped.reshape(B, K, Cc, H, W), mask.reshape(B, K, H, W))
+
+    def _warp_planes(self, src_feats, src_extrinsics, src_Ks, cur_invK, depth_planes_bdhw, D, B, K, Cc,
+                     want_pix):
+        """Both ``warp_features`` methods: one ``srcv_warp_features_planes_f32`` call over the first ``D``
+        planes of ``depth_planes_bdhw``.  Returns ``(warped (B,K,D,C,H,W), depths (B,K,D,H,W),
+        mask (B,K,D,H,W), pix (B,K,D,2,H,W) or None, cur_invK as fp32)``."""
         lib = _native.load()
         dev = src_feats.device
         _require_cuda(dev)
-        B, K, Cc = batch_size, num_src_frames, num_feat_channels
         H, W = self.matching_height, self.matching_width
         src = _f32c(src_feats, "src_feats", dev).reshape(B, K, Cc, H, W)
         E, Ks = _f32c(src_extrinsics, "src_extrinsics", dev), _f32c(src_Ks, "src_Ks", dev)
         invK = _f32c(cur_invK, "cur_invK", dev)
-        plane = _plane_table(depth_plane_b1hw, 1)
-        shape = _native.Shape(B, K, Cc, H, W, 1)
+        planes = _f32c(_plane_table(depth_planes_bdhw, D), "depth plane", dev)
+        shape = _native.Shape(B, K, Cc, H, W, D)
         cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
         with torch.cuda.device(dev):
-            warped = torch.empty(B, K, Cc, H, W, device=dev, dtype=torch.float32)
-            depths = torch.empty(B, K, H, W, device=dev, dtype=torch.float32)
-            mask = torch.empty(B, K, H, W, device=dev, dtype=torch.float32)
+            warped = torch.empty(B, K, D, Cc, H, W, device=dev, dtype=torch.float32)
+            depths = torch.empty(B, K, D, H, W, device=dev, dtype=torch.float32)
+            mask = torch.empty(B, K, D, H, W, device=dev, dtype=torch.float32)
+            pix = torch.empty(B, K, D, 2, H, W, device=dev, dtype=torch.float32) if want_pix else None
             n = lib.srcv_warp_workspace_bytes(C.byref(shape))
             ws = torch.empty(n, device=dev, dtype=torch.uint8)
-            _native.check(lib.srcv_warp_features_f32(
-                C.byref(shape), _ptr(src), C.byref(cams), _ptr(plane), int(plane.dim() == 4), _ptr(warped),
-                _ptr(depths), _ptr(mask), _ptr(ws), n,
+            _native.check(lib.srcv_warp_features_planes_f32(
+                C.byref(shape), _ptr(src), C.byref(cams), _ptr(planes), int(planes.dim() == 4), _ptr(warped),
+                _ptr(depths), _ptr(mask), _ptr(pix), _ptr(ws), n,
                 C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-        world_points_b4N = self.backprojector(depth_plane_b1hw.expand(B, 1, H, W), invK)
-        return world_points_b4N.repeat_interleave(K, dim=0), depths, warped, mask
+        return warped, depths, mask, pix, invK
 
     # -- reference :338-342 ---------------------------------------------------
     def indices_to_disparity(self, indices, depth_planes_bdhw):
@@ -378,20 +387,10 @@ class CostVolumeManager(nn.Module):
 
     def _run_fused(self, cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, min_depth,
                    max_depth, depth_planes_bdhw, want_lowest, allow_grad=False, raw_poses=None):
-        lib = _native.load()
-        dev, shape, t, cams, pl, planes_ret, keep = self._prepare(
+        _, shape, t, cams, pl, planes_ret, keep = self._prepare(
             cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, min_depth,
             max_depth, depth_planes_bdhw, need_poses=False, allow_grad=allow_grad, raw_poses=raw_poses)
-        with torch.cuda.device(dev):
-            cost = torch.empty(shape.B, shape.D, shape.H, shape.W, device=dev, dtype=torch.float32)
-            lowest = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.float32) \
-                if want_lowest else None
-            nbytes = lib.srcv_dot_workspace_bytes(C.byref(shape))
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            _native.check(lib.srcv_dot_forward_f32(
-                C.byref(shape), _ptr(t["cur"]), _ptr(t["src"]), C.byref(cams), C.byref(pl),
-                _ptr(cost), _ptr(lowest), _ptr(ws), nbytes, C.c_void_p(stream)))
+        cost, lowest = torch_ops._dot_sweep(shape, t["cur"], t["src"], cams, pl, want_lowest)
         return cost, lowest, planes_ret, None
 
     # -- reference :345-380 ---------------------------------------------------
@@ -497,30 +496,14 @@ class FeatureVolumeManager(CostVolumeManager):
 
     def _run_fused(self, cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, min_depth,
                    max_depth, depth_planes_bdhw, return_mask, want_lowest, allow_grad=False, raw_poses=None):
-        lib = _native.load()
         dev, shape, t, cams, pl, planes_ret, keep = self._prepare(
             cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, min_depth,
             max_depth, depth_planes_bdhw, need_poses=True, allow_grad=allow_grad, raw_poses=raw_poses)
         n_features = shape.C * (shape.K + 1) + 10 * shape.K + 4
         w, wkeep = self._mlp_weights(dev, n_features)
         wkeep.append(self._attach_packed_image(dev, shape, w, wkeep))
-        with torch.cuda.device(dev):
-            cost = torch.empty(shape.B, shape.D, shape.H, shape.W, device=dev, dtype=torch.float32)
-            lowest = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.float32) \
-                if want_lowest else None
-            mask = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.uint8) \
-                if return_mask else None
-            nbytes = lib.srcv_mlp_workspace_bytes(C.byref(shape), C.byref(w))
-            if nbytes == 0:
-                raise NotImplementedError(
-                    f"MLP widths ({w.hidden1},{w.hidden2}) are not supported by the fused kernels")
-            ws = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-            stream = torch.cuda.current_stream(dev).cuda_stream
-            _native.check(lib.srcv_mlp_forward_f32(
-                C.byref(shape), _ptr(t["cur"]), _ptr(t["src"]), C.byref(cams), C.byref(pl),
-                C.byref(w), _ptr(cost), _ptr(lowest), _ptr(mask), _ptr(ws), nbytes,
-                C.c_void_p(stream)))
-        return cost, lowest, planes_ret, (mask.bool() if mask is not None else None)
+        cost, lowest, mask = torch_ops._mlp_sweep(shape, t["cur"], t["src"], cams, pl, w, want_lowest, return_mask)
+        return cost, lowest, planes_ret, mask
 
     # -- reference :739-746 ---------------------------------------------------
     def to_fast(self) -> "FastFeatureVolumeManager":
@@ -552,29 +535,11 @@ class FastFeatureVolumeManager(FeatureVolumeManager):
         form (550 MB per frame at the hero shape) the fused sweep avoids; it exists because the
         reference exposes it.  ``uv_scale`` is accepted and unused (the kernel works in pixel
         coordinates)."""
-        lib = _native.load()
-        dev = src_feats.device
-        _require_cuda(dev)
         B, K, Cc = batch_size, num_src_frames, num_feat_channels
         H, W = self.matching_height, self.matching_width
         D = depth_plane_bdhw.shape[1]
-        src = _f32c(src_feats, "src_feats", dev).reshape(B, K, Cc, H, W)
-        E, Ks = _f32c(src_extrinsics, "src_extrinsics", dev), _f32c(src_Ks, "src_Ks", dev)
-        invK = _f32c(cur_invK, "cur_invK", dev)
-        planes = _f32c(_plane_table(depth_plane_bdhw, D), "depth_plane_bdhw", dev)
-        shape = _native.Shape(B, K, Cc, H, W, D)
-        cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
-        with torch.cuda.device(dev):
-            warped = torch.empty(B, K, D, Cc, H, W, device=dev, dtype=torch.float32)
-            depths = torch.empty(B, K, D, H, W, device=dev, dtype=torch.float32)
-            mask = torch.empty(B, K, D, H, W, device=dev, dtype=torch.float32)
-            pix = torch.empty(B, K, D, 2, H, W, device=dev, dtype=torch.float32)
-            n = lib.srcv_warp_workspace_bytes(C.byref(shape))
-            ws = torch.empty(n, device=dev, dtype=torch.uint8)
-            _native.check(lib.srcv_warp_features_planes_f32(
-                C.byref(shape), _ptr(src), C.byref(cams), _ptr(planes), int(planes.dim() == 4), _ptr(warped),
-                _ptr(depths), _ptr(mask), _ptr(pix), _ptr(ws), n,
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+        warped, depths, mask, pix, invK = self._warp_planes(src_feats, src_extrinsics, src_Ks, cur_invK,
+                                                            depth_plane_bdhw, D, B, K, Cc, want_pix=True)
         # world points of every plane (:857-873): X = depth * (invK3 @ p), homogeneous
         world = self.backprojector(depth_plane_bdhw.reshape(B * D, 1, H, W).expand(B * D, 1, H, W),
                                    invK.repeat_interleave(D, dim=0))

@@ -89,29 +89,73 @@ def _planes_struct(planes: Tensor, per_pixel: bool) -> _native.Planes:
     return pl
 
 
-# ---------------------------------------------------------------------------------------------
-# b200cv::dot_forward / dot_backward
-# ---------------------------------------------------------------------------------------------
-@torch.library.custom_op("b200cv::dot_forward", mutates_args=(), device_types="cuda")
-def dot_forward(cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor, src_Ks: Tensor,
-                cur_invK: Tensor, planes: Tensor) -> Tuple[Tensor, Tensor]:
-    """``(cost (B,D,H,W), lowest_cost (B,H,W))`` of the dot-product sweep."""
-    B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes)
-    lib = _native.load()
-    dev = src_feats.device
+def _marshal(cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor, src_Ks: Tensor, cur_invK: Tensor,
+             planes: Tensor, src_poses: Tensor | None = None):
+    """Checks the operator arguments (``_check_shapes``) and lays them out for the C ABI: returns
+    ``(shape, cams, planes_struct, tensors)``, ``tensors`` being the dense, 16-byte aligned copies
+    ``(cur, src, E, P, Ks, invK, planes)`` the structs point into (``P`` None without poses); they must
+    stay alive until the call returns."""
+    B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
+                                                 planes, src_poses)
     cur, src, E, Ks, invK, pln = map(_c16, (cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes))
-    shape = _native.Shape(B, K, Cc, H, W, D)
-    cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
-    pl = _planes_struct(pln, per_pixel)
+    P = _c16(src_poses) if src_poses is not None else None
+    cams = _native.Cameras(E.data_ptr(), P.data_ptr() if P is not None else None, Ks.data_ptr(), invK.data_ptr())
+    return _native.Shape(B, K, Cc, H, W, D), cams, _planes_struct(pln, per_pixel), (cur, src, E, P, Ks, invK, pln)
+
+
+# ---------------------------------------------------------------------------------------------
+# the forward launches of both the operators and the managers (their callers check the arguments)
+# ---------------------------------------------------------------------------------------------
+def _dot_sweep(shape: _native.Shape, cur: Tensor, src: Tensor, cams: _native.Cameras, pl: _native.Planes,
+               want_lowest: bool) -> Tuple[Tensor, Tensor | None]:
+    """``(cost (B,D,H,W), lowest_cost (B,H,W) or None)``: one ``srcv_dot_forward_f32`` call on the
+    current stream of ``src``'s device."""
+    lib = _native.load()
+    dev = src.device
     with torch.cuda.device(dev):
-        cost = torch.empty(B, D, H, W, device=dev, dtype=torch.float32)
-        lowest = torch.empty(B, H, W, device=dev, dtype=torch.float32)
+        cost = torch.empty(shape.B, shape.D, shape.H, shape.W, device=dev, dtype=torch.float32)
+        lowest = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.float32) if want_lowest else None
         n = lib.srcv_dot_workspace_bytes(C.byref(shape))
         ws = torch.empty(n, device=dev, dtype=torch.uint8)
         _native.check(lib.srcv_dot_forward_f32(
             C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), _ptr(cost), _ptr(lowest),
             _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
     return cost, lowest
+
+
+def _mlp_sweep(shape: _native.Shape, cur: Tensor, src: Tensor, cams: _native.Cameras, pl: _native.Planes,
+               w: _native.MlpWeights, want_lowest: bool, want_mask: bool
+               ) -> Tuple[Tensor, Tensor | None, Tensor | None]:
+    """``(cost (B,D,H,W), lowest_cost (B,H,W) or None, overall_mask (B,H,W) bool or None)``: one
+    ``srcv_mlp_forward_f32`` call on the current stream of ``src``'s device.  Without
+    ``w.packed_image`` the tensor-core kernel packs the weights into its workspace."""
+    lib = _native.load()
+    dev = src.device
+    with torch.cuda.device(dev):
+        cost = torch.empty(shape.B, shape.D, shape.H, shape.W, device=dev, dtype=torch.float32)
+        lowest = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.float32) if want_lowest else None
+        mask = torch.empty(shape.B, shape.H, shape.W, device=dev, dtype=torch.uint8) if want_mask else None
+        n = lib.srcv_mlp_workspace_bytes(C.byref(shape), C.byref(w))
+        if n == 0:
+            raise NotImplementedError(f"MLP widths ({w.hidden1},{w.hidden2}) are not supported by the fused kernels")
+        ws = torch.empty(n, device=dev, dtype=torch.uint8)
+        _native.check(lib.srcv_mlp_forward_f32(
+            C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), C.byref(w), _ptr(cost),
+            _ptr(lowest), _ptr(mask), _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+    return cost, lowest, (mask.bool() if mask is not None else None)
+
+
+# ---------------------------------------------------------------------------------------------
+# b200cv::dot_forward / dot_backward
+# ---------------------------------------------------------------------------------------------
+def _dot_forward(cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor, src_Ks: Tensor,
+                 cur_invK: Tensor, planes: Tensor) -> Tuple[Tensor, Tensor]:
+    """``(cost (B,D,H,W), lowest_cost (B,H,W))`` of the dot-product sweep."""
+    shape, cams, pl, (cur, src, *keep) = _marshal(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes)
+    return _dot_sweep(shape, cur, src, cams, pl, want_lowest=True)
+
+
+dot_forward = torch.library.custom_op("b200cv::dot_forward", _dot_forward, mutates_args=(), device_types="cuda")
 
 
 @dot_forward.register_fake
@@ -123,16 +167,13 @@ def _(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes):
 def _dot_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor,
                   src_Ks: Tensor, cur_invK: Tensor, planes: Tensor) -> Tuple[Tensor, Tensor]:
     """``(dL/dcur_feats, dL/dsrc_feats)`` given ``dL/dcost``."""
-    B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes)
-    if tuple(grad_cost.shape) != (B, D, H, W) or grad_cost.dtype != torch.float32:
-        raise ValueError(f"grad_cost must be float32 {(B, D, H, W)}")
+    shape, cams, pl, (cur, src, *keep) = _marshal(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes)
+    bdhw = (shape.B, shape.D, shape.H, shape.W)
+    if tuple(grad_cost.shape) != bdhw or grad_cost.dtype != torch.float32:
+        raise ValueError(f"grad_cost must be float32 {bdhw}")
     lib = _native.load()
-    dev = src_feats.device
-    g, cur, src, E, Ks, invK, pln = map(
-        _c16, (grad_cost, cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK, planes))
-    shape = _native.Shape(B, K, Cc, H, W, D)
-    cams = _native.Cameras(E.data_ptr(), None, Ks.data_ptr(), invK.data_ptr())
-    pl = _planes_struct(pln, per_pixel)
+    dev = src.device
+    g = _c16(grad_cost)
     with torch.cuda.device(dev):
         gcur, gsrc = torch.empty_like(cur), torch.empty_like(src)
         n = lib.srcv_dot_backward_workspace_bytes(C.byref(shape))
@@ -190,36 +231,20 @@ def _check_mlp(K: int, Cc: int, w1, b1, w2, b2, w3, b3) -> Tuple[int, int]:
     return h1, h2
 
 
-@torch.library.custom_op("b200cv::mlp_forward", mutates_args=(), device_types="cuda")
-def mlp_forward(cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor, src_poses: Tensor,
-                src_Ks: Tensor, cur_invK: Tensor, planes: Tensor, w1: Tensor, b1: Tensor, w2: Tensor,
-                b2: Tensor, w3: Tensor, b3: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
+def _mlp_forward(cur_feats: Tensor, src_feats: Tensor, src_extrinsics: Tensor, src_poses: Tensor,
+                 src_Ks: Tensor, cur_invK: Tensor, planes: Tensor, w1: Tensor, b1: Tensor, w2: Tensor,
+                 b2: Tensor, w3: Tensor, b3: Tensor) -> Tuple[Tensor, Tensor, Tensor]:
     """``(cost (B,D,H,W), lowest_cost (B,H,W), overall_mask (B,H,W) bool)`` of the metadata-MLP
     sweep; the MLP is ``F→H1→H2→1`` with LeakyReLU(0.01) (modules/networks.py:129-147)."""
-    B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
-                                                 planes, src_poses)
-    h1, h2 = _check_mlp(K, Cc, w1, b1, w2, b2, w3, b3)
-    lib = _native.load()
-    dev = src_feats.device
-    cur, src, E, P, Ks, invK, pln = map(
-        _c16, (cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, planes))
+    shape, cams, pl, (cur, src, *keep) = _marshal(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
+                                                  planes, src_poses)
+    h1, h2 = _check_mlp(shape.K, shape.C, w1, b1, w2, b2, w3, b3)
     ws_t = [_c16(t.detach()) for t in (w1, b1, w2, b2, w3, b3)]
-    shape = _native.Shape(B, K, Cc, H, W, D)
-    cams = _native.Cameras(E.data_ptr(), P.data_ptr(), Ks.data_ptr(), invK.data_ptr())
-    pl = _planes_struct(pln, per_pixel)
     w = _native.MlpWeights(*[t.data_ptr() for t in ws_t], h1, h2)
-    with torch.cuda.device(dev):
-        cost = torch.empty(B, D, H, W, device=dev, dtype=torch.float32)
-        lowest = torch.empty(B, H, W, device=dev, dtype=torch.float32)
-        mask = torch.empty(B, H, W, device=dev, dtype=torch.uint8)
-        n = lib.srcv_mlp_workspace_bytes(C.byref(shape), C.byref(w))
-        if n == 0:
-            raise NotImplementedError(f"MLP widths ({h1},{h2}) are not supported by the fused kernels")
-        ws = torch.empty(n, device=dev, dtype=torch.uint8)
-        _native.check(lib.srcv_mlp_forward_f32(
-            C.byref(shape), _ptr(cur), _ptr(src), C.byref(cams), C.byref(pl), C.byref(w), _ptr(cost),
-            _ptr(lowest), _ptr(mask), _ptr(ws), n, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-    return cost, lowest, mask.bool()
+    return _mlp_sweep(shape, cur, src, cams, pl, w, want_lowest=True, want_mask=True)
+
+
+mlp_forward = torch.library.custom_op("b200cv::mlp_forward", _mlp_forward, mutates_args=(), device_types="cuda")
 
 
 @mlp_forward.register_fake
@@ -237,19 +262,16 @@ def _mlp_backward(grad_cost: Tensor, cur_feats: Tensor, src_feats: Tensor, src_e
                   ) -> Tuple[Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor, Tensor]:
     """``(dL/dcur_feats, dL/dsrc_feats, dL/dw1, dL/db1, dL/dw2, dL/db2, dL/dw3, dL/db3)`` given
     ``dL/dcost`` — a recompute kernel: nothing of the forward is needed but its inputs."""
-    B, K, Cc, H, W, D, per_pixel = _check_shapes(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
-                                                 planes, src_poses)
-    h1, h2 = _check_mlp(K, Cc, w1, b1, w2, b2, w3, b3)
-    if tuple(grad_cost.shape) != (B, D, H, W) or grad_cost.dtype != torch.float32:
-        raise ValueError(f"grad_cost must be float32 {(B, D, H, W)}")
+    shape, cams, pl, (cur, src, *keep) = _marshal(cur_feats, src_feats, src_extrinsics, src_Ks, cur_invK,
+                                                  planes, src_poses)
+    h1, h2 = _check_mlp(shape.K, shape.C, w1, b1, w2, b2, w3, b3)
+    bdhw = (shape.B, shape.D, shape.H, shape.W)
+    if tuple(grad_cost.shape) != bdhw or grad_cost.dtype != torch.float32:
+        raise ValueError(f"grad_cost must be float32 {bdhw}")
     lib = _native.load()
-    dev = src_feats.device
-    g, cur, src, E, P, Ks, invK, pln = map(
-        _c16, (grad_cost, cur_feats, src_feats, src_extrinsics, src_poses, src_Ks, cur_invK, planes))
+    dev = src.device
+    g = _c16(grad_cost)
     ws_t = [_c16(t.detach()) for t in (w1, b1, w2, b2, w3, b3)]
-    shape = _native.Shape(B, K, Cc, H, W, D)
-    cams = _native.Cameras(E.data_ptr(), P.data_ptr(), Ks.data_ptr(), invK.data_ptr())
-    pl = _planes_struct(pln, per_pixel)
     w = _native.MlpWeights(*[t.data_ptr() for t in ws_t], h1, h2)
     with torch.cuda.device(dev):
         gcur, gsrc = torch.empty_like(cur), torch.empty_like(src)
