@@ -505,6 +505,35 @@ int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* args, const float* 
                                   float* kept, int64_t* num_kept, void* workspace, size_t workspace_bytes,
                                   void* stream);
 
+/* ---- voxel down-sampling (DESIGN §4.19) --------------------------------------------------- *
+ * Open3D's VoxelDownSample rule, in fp64 from the fp32 points (metres) and voxel size s:
+ *   b = min_i p_i - 0.5 s per axis;  voxel of p: v = floor((p - b) / s), an IEEE subtraction and division;
+ *   each occupied voxel's point is the fp64 sum of its points, accumulated in input order from 0.0, divided by
+ *   their count and rounded once to fp32; colours likewise (uint8 taken as c / 255.0 in fp64, floats as given).
+ * srcv_voxel_down_sample_f32: points (num_points,3) f32 and colors (num_points,3) of color_type (NULL for
+ *   SRCV_COLORS_NONE), DEVICE.  out_points (num_points,3) f32, out_colors (num_points,3) f32 (NULL without
+ *   colours) and out_counts (num_points) int32 out: the first M rows, one per occupied voxel in ascending
+ *   (vx, vy, vz) order; num_out DEVICE int64 out = M.  A stable LSD radix sort of the voxel keys with as many
+ *   8-bit passes as the extent needs: bitwise deterministic, independent of thread timing and input order.
+ *   49 launches; the sort passes the extent does not need exit at once.
+ * flags: DEVICE uint32 the caller zeroes; ORs SRCV_MESH_EVAL_NONFINITE (a non-finite coordinate),
+ *   SRCV_VOXEL_NONFINITE_COLOR (a non-finite colour) and SRCV_VOXEL_EXTENT (2^21 or more voxels on an axis).
+ *   Once a coordinate or extent bit is set no output row is written.
+ * Limits (SRCV_ERR_SHAPE): 1 <= num_points <= 2^28; s finite and > 0.  The workspace (about 40 bytes per point)
+ * is sized by srcv_voxel_down_sample_workspace_bytes (0 outside the limits).  Nothing synchronises with the
+ * host.                                                                                                      */
+#define SRCV_VOXEL_NONFINITE_COLOR 16u
+#define SRCV_VOXEL_EXTENT 32u
+#define SRCV_COLORS_NONE 0
+#define SRCV_COLORS_U8 1
+#define SRCV_COLORS_F32 2
+#define SRCV_COLORS_F64 3
+size_t srcv_voxel_down_sample_workspace_bytes(int64_t num_points);
+int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, double voxel_size, const void* colors,
+                                   int32_t color_type, float* out_points, float* out_colors, int32_t* out_counts,
+                                   int64_t* num_out, uint32_t* flags, void* workspace, size_t workspace_bytes,
+                                   void* stream);
+
 /* ---- multi-view depth consistency (point-cloud fusion) ------------------------------ *
  * Replaces process_depth of the reference's 3DVNet-style fuser (tools/torch_point_cloud_fusion.py
  * :12-97), which pc_fusion.py:158 runs for every frame of a scan against all the others: for each

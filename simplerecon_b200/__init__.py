@@ -28,3 +28,4 @@ from .metrics import compute_depth_metrics, compute_depth_metrics_batched, depth
 from .normals import NormalGenerator, NormalsLoss  # noqa: E402,F401  (reference geometry_utils.py:92-133, losses.py:57-77)
 from .mesh_eval import mesh_metrics, nearest_distances, sample_surface  # noqa: E402,F401  (mesh metrics, DESIGN §4.17)
 from .mesh_eval import Views, observation_counts  # noqa: E402,F401  (visibility culling, DESIGN §4.18)
+from .point_cloud_fusion import fuse_point_cloud, voxel_down_sample  # noqa: E402,F401  (pc_fusion.py:158-169, DESIGN §4.19)

@@ -125,6 +125,8 @@ class MeshEvalArgs(C.Structure):
 
 
 MESH_EVAL_BAD_FACE, MESH_EVAL_NONFINITE, MESH_EVAL_ZERO_AREA, MESH_EVAL_BAD_VIEW = 1, 2, 4, 8
+VOXEL_NONFINITE_COLOR, VOXEL_EXTENT = 16, 32
+COLORS_NONE, COLORS_U8, COLORS_F32, COLORS_F64 = 0, 1, 2, 3
 
 
 class MeshViews(C.Structure):
@@ -194,6 +196,9 @@ SYMBOLS = {
     "srcv_mesh_metrics_f64": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, C.c_double, _fp, _fp, C.c_size_t, _fp]),
     "srcv_observation_counts_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), C.POINTER(MeshViews), _fp, _fp, _fp]),
     "srcv_compact_observed_f32": (C.c_int32, [C.POINTER(MeshEvalArgs), _fp, _fp, _fp, _fp, _fp, C.c_size_t, _fp]),
+    "srcv_voxel_down_sample_workspace_bytes": (C.c_size_t, [C.c_int64]),
+    "srcv_voxel_down_sample_f32": (C.c_int32, [_fp, C.c_int64, C.c_double, _fp, C.c_int32, _fp, _fp, _fp, _fp, _fp, _fp,
+                                               C.c_size_t, _fp]),
     "srcv_mvs_workspace_bytes": (C.c_size_t, [C.POINTER(MvsScan)]),
     "srcv_mvs_consistency_f32": (C.c_int32, [C.POINTER(MvsScan), C.c_int32, C.c_float, C.c_int32, _fp, _fp, _fp,
                                              _fp, C.c_size_t, C.c_int32, _fp]),

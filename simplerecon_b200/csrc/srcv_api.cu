@@ -834,6 +834,39 @@ int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* a, const float* poi
   return SRCV_OK;
 }
 
+size_t srcv_voxel_down_sample_workspace_bytes(int64_t num_points) {
+  if (num_points < 1 || num_points > kMeshEvalMaxPoints) return 0;
+  return voxel_down_sample_workspace_bytes(num_points);
+}
+
+int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, double voxel_size, const void* colors,
+                                   int32_t color_type, float* out_points, float* out_colors, int32_t* out_counts,
+                                   int64_t* num_out, uint32_t* flags, void* workspace, size_t workspace_bytes,
+                                   void* stream_) {
+  if (!points || !out_points || !out_counts || !num_out || !flags)
+    return fail(SRCV_ERR_NULL, "points / out_points / out_counts / num_out / flags is NULL");
+  if (num_points < 1 || num_points > kMeshEvalMaxPoints)
+    return fail(SRCV_ERR_SHAPE, "bad point count num_points=%lld (1 .. 2^28)", (long long)num_points);
+  if (!(voxel_size > 0.0 && std::isfinite(voxel_size)))
+    return fail(SRCV_ERR_SHAPE, "voxel_size must be finite and > 0, got %g", voxel_size);
+  if (color_type < SRCV_COLORS_NONE || color_type > SRCV_COLORS_F64)
+    return fail(SRCV_ERR_UNSUPPORTED, "unknown color_type %d", color_type);
+  if ((color_type != SRCV_COLORS_NONE) != (colors != nullptr && out_colors != nullptr))
+    return fail(SRCV_ERR_NULL, "colors and out_colors must be given exactly when color_type is not SRCV_COLORS_NONE");
+  const uintptr_t csize = color_type == SRCV_COLORS_F64 ? 8u : color_type == SRCV_COLORS_F32 ? 4u : 1u;
+  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(out_points) |
+        reinterpret_cast<uintptr_t>(out_colors) | reinterpret_cast<uintptr_t>(out_counts) |
+        reinterpret_cast<uintptr_t>(flags)) & 3u) != 0 || (reinterpret_cast<uintptr_t>(num_out) & 7u) != 0 ||
+      (reinterpret_cast<uintptr_t>(colors) & (csize - 1u)) != 0)
+    return fail(SRCV_ERR_UNSUPPORTED, "misaligned point, colour, count or flag arrays");
+  if (int32_t e = check_workspace(workspace, workspace_bytes, voxel_down_sample_workspace_bytes(num_points))) return e;
+  g_last_variant.store("voxel_down_sample_f32");
+  cudaError_t err = launch_voxel_down_sample(points, num_points, voxel_size, colors, color_type, out_points, out_colors,
+                                             out_counts, num_out, flags, workspace, static_cast<cudaStream_t>(stream_));
+  if (err != cudaSuccess) return cuda_fail(err, "voxel_down_sample");
+  return SRCV_OK;
+}
+
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {
   if (!s || s->N <= 0) return 0;
   return mvs_workspace_bytes(s->N);

@@ -152,6 +152,11 @@ cudaError_t launch_observation_counts(const srcv_mesh_eval_args& a, const srcv_m
                                       int32_t* counts, cudaStream_t stream);
 cudaError_t launch_compact_observed(const srcv_mesh_eval_args& a, const float* points, const int32_t* counts,
                                     float* kept, int64_t* num_kept, void* workspace, cudaStream_t stream);
+// voxel down-sampling of a point cloud (csrc/srcv_voxel_downsample.cuh, in the srcv_tsdf.cu unit)
+size_t voxel_down_sample_workspace_bytes(long long n);
+cudaError_t launch_voxel_down_sample(const float* points, long long n, double voxel_size, const void* colors,
+                                     int color_type, float* out_points, float* out_colors, int32_t* out_counts,
+                                     int64_t* num_out, unsigned* flags, void* workspace, cudaStream_t stream);
 
 // multi-view depth consistency (csrc/srcv_mvs.cu)
 size_t mvs_workspace_bytes(int n);

@@ -745,3 +745,6 @@ cudaError_t launch_mesh_metrics(const srcv_mesh_eval_args& a, const double* dist
 
 // visibility culling of the evaluated points (DESIGN §4.18), built on this file's scan and helpers
 #include "srcv_mesh_visibility.cuh"
+
+// voxel down-sampling of point clouds (DESIGN §4.19), built on this file's box partials and scan
+#include "srcv_voxel_downsample.cuh"

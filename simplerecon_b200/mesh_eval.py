@@ -9,7 +9,9 @@ queue for far queries) and a fixed-order fp64 reduction.
 
 Parity with TransformerFusion's or NeuralRecon's scripts is not claimed: their code is not part of the
 reference, and they may apply visibility masks or voxel down-sampling in ways this module does not reproduce.
-Voxel down-sampling is not done here.
+``mesh_metrics(..., down_sample=s)`` voxel-down-samples both point sets at voxel size ``s`` before scoring them
+(``point_cloud_fusion.voxel_down_sample``, csrc/srcv_voxel_downsample.cuh, DESIGN §4.19), which approximates the
+2 cm down-sampling NeuralRecon's evaluation is commonly run with.
 
 Visibility culling (csrc/srcv_mesh_visibility.cuh, DESIGN §4.18): given the depth frames of the scan
 (``Views``), ``observation_counts`` counts the frames that observe each point, and ``mesh_metrics(..., views=)``
@@ -45,7 +47,10 @@ _MAX_POINTS = 1 << 28
 _FLAG_NAMES = ((_native.MESH_EVAL_BAD_FACE, "a face index outside [0, V)"),
                (_native.MESH_EVAL_NONFINITE, "a non-finite (NaN or inf) coordinate"),
                (_native.MESH_EVAL_ZERO_AREA, "a mesh of zero total area"),
-               (_native.MESH_EVAL_BAD_VIEW, "a non-finite entry in a view's K or cam_T_world"))
+               (_native.MESH_EVAL_BAD_VIEW, "a non-finite entry in a view's K or cam_T_world"),
+               (_native.VOXEL_NONFINITE_COLOR, "a non-finite (NaN or inf) colour"),
+               (_native.VOXEL_EXTENT, "an extent of 2^21 or more voxels on an axis (the voxel size is too small)"))
+_COLOR_TYPES = {torch.uint8: _native.COLORS_U8, torch.float32: _native.COLORS_F32, torch.float64: _native.COLORS_F64}
 
 
 def _require_cuda(t: torch.Tensor) -> None:
@@ -263,6 +268,47 @@ def _compact(points, counts, flags, num_kept) -> torch.Tensor:
     return out
 
 
+def _check_voxel_size(voxel_size) -> float:
+    s = float(voxel_size)
+    if not (math.isfinite(s) and s > 0.0):
+        raise ValueError(f"voxel_size must be finite and > 0, got {voxel_size}")
+    return s
+
+
+def _colors(x, points) -> torch.Tensor:
+    """(N, 3) uint8, float32 or float64 colours on the points' device, as given (no conversion)."""
+    t = _tensor(x, "colors")
+    if t.device != points.device:
+        raise ValueError(f"colors on {t.device} and points on {points.device}")
+    if tuple(t.shape) != (points.shape[0], 3):
+        raise ValueError(f"colors must be ({points.shape[0]}, 3) like the points, got {tuple(t.shape)}")
+    if t.dtype not in _COLOR_TYPES:
+        raise ValueError(f"colors must be uint8, float32 or float64, got {t.dtype}")
+    return t.detach().contiguous()
+
+
+def _down_sample(points, voxel_size: float, flags, colors=None, num_out=None):
+    """Launches the voxel down-sampling of ``points`` (fp32 (N, 3) on the device): returns (points (N, 3) fp32,
+    colours (N, 3) fp32 or None, counts (N,) int32, num_out (1,) int64), of which the first num_out rows are the
+    result.  No host synchronisation."""
+    dev = points.device
+    n = points.shape[0]
+    lib = _lib()
+    ws = torch.empty(lib.srcv_voxel_down_sample_workspace_bytes(n), dtype=torch.uint8, device=dev)
+    out = torch.empty(n, 3, dtype=torch.float32, device=dev)
+    out_c = torch.empty(n, 3, dtype=torch.float32, device=dev) if colors is not None else None
+    counts = torch.empty(n, dtype=torch.int32, device=dev)
+    if num_out is None:
+        num_out = torch.zeros(1, dtype=torch.int64, device=dev)
+    ptr = lambda t: C.c_void_p(t.data_ptr()) if t is not None else None   # noqa: E731
+    with torch.cuda.device(dev):
+        _native.check(lib.srcv_voxel_down_sample_f32(
+            ptr(points), n, float(voxel_size), ptr(colors),
+            _native.COLORS_NONE if colors is None else _COLOR_TYPES[colors.dtype], ptr(out), ptr(out_c), ptr(counts),
+            ptr(num_out), ptr(flags), ptr(ws), ws.numel(), _stream(dev)))
+    return out, out_c, counts, num_out
+
+
 def _observation_counts(points, depths, K, cam_T_world, margin=0.05, max_depth=math.inf, counts=None,
                         tile_cull: bool = True, stats=None) -> torch.Tensor:
     p = _coords(points, "points")
@@ -294,7 +340,7 @@ def observation_counts(points, depths, K, cam_T_world, margin: float = 0.05, max
 
 
 def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_NUM_SAMPLES, seed: int = 0,
-                 views: Views | None = None) -> dict:
+                 views: Views | None = None, down_sample: float | None = None) -> dict:
     """{acc, comp, chamfer, precision, recall, fscore} (Python floats, in that order) of ``pred`` against ``gt``.
 
     Each side is a mesh ``(verts, faces)``, replaced by ``num_samples`` area-uniform surface samples
@@ -305,16 +351,28 @@ def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_N
 
     With ``views`` (``Views``), each side's points that no frame observes (``observation_counts`` == 0) are
     dropped before the distances; the call then synchronises twice, and a side left with no point, or a view with
-    a non-finite K or cam_T_world entry, raises ``ValueError``."""
+    a non-finite K or cam_T_world entry, raises ``ValueError``.
+
+    With ``down_sample`` (a voxel size in metres, e.g. 0.02), each side's points (its samples, or the point set as
+    given) are replaced by their voxel down-sampling (``point_cloud_fusion.voxel_down_sample``) before the views and
+    the distances; this adds one host synchronisation, and a side whose extent is 2^21 voxels or more raises
+    ``ValueError``.  ``None`` (the default) scores the points as they are."""
     if not threshold > 0:
         raise ValueError(f"threshold must be positive, got {threshold}")
     n = _check_count(num_samples)
+    voxel = None if down_sample is None else _check_voxel_size(down_sample)
     flags = torch.zeros(1, dtype=torch.int32, device=_device_of(pred, "pred"))
     P = _side(pred, "pred", n, int(seed), flags)
     G = _side(gt, "gt", n, int(seed) + 1, flags)
     if P.device != G.device:
         raise ValueError(f"pred on {P.device} and gt on {G.device}")
     dev = P.device
+    if voxel is not None:
+        num_out = torch.zeros(2, dtype=torch.int64, device=dev)
+        ds = [_down_sample(X, voxel, flags, num_out=num_out[k:k + 1])[0] for k, X in enumerate((P, G))]
+        n_pred, n_gt, bad = torch.cat([num_out, flags.to(torch.int64)]).tolist()   # the extra host synchronisation
+        _raise_flags(bad)
+        P, G = ds[0][:n_pred], ds[1][:n_gt]
     if views is not None:
         vs, keep = _views(views, dev)
         num_kept = torch.zeros(2, dtype=torch.int64, device=dev)
@@ -343,6 +401,6 @@ def mesh_metrics(pred, gt, threshold: float = 0.05, num_samples: int = DEFAULT_N
     return dict(zip(KEYS, vals[:6]))
 
 
-def _raise_flags(bad: int) -> None:
+def _raise_flags(bad: int, who: str = "mesh_metrics") -> None:
     if bad:
-        raise ValueError("mesh_metrics: the input has " + " and ".join(name for bit, name in _FLAG_NAMES if bad & bit))
+        raise ValueError(f"{who}: the input has " + " and ".join(name for bit, name in _FLAG_NAMES if bad & bit))

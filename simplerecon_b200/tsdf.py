@@ -380,12 +380,13 @@ def colors_to_u8(colors) -> np.ndarray:
     return np.rint(np.float32(255.0) * np.clip(c.astype(np.float32), 0.0, 1.0)).astype(np.uint8)
 
 
-def write_ply(path, verts: np.ndarray, faces: np.ndarray, colors: np.ndarray | None = None) -> None:
+def write_ply(path, verts: np.ndarray, faces: np.ndarray | None, colors: np.ndarray | None = None) -> None:
     """Binary little-endian PLY: float x, y, z (and uchar red, green, blue when ``colors`` is given:
     uint8 as is, floats in [0, 1] through ``colors_to_u8``) per vertex; a uchar count and int indices per
-    face."""
+    face.  ``faces=None`` writes a point cloud: no face element at all (``read_ply`` returns faces=None)."""
     verts = np.ascontiguousarray(verts, dtype="<f4").reshape(-1, 3)
-    faces = np.ascontiguousarray(faces, dtype="<i4").reshape(-1, 3)
+    if faces is not None:
+        faces = np.ascontiguousarray(faces, dtype="<i4").reshape(-1, 3)
     vprops = "property float x\nproperty float y\nproperty float z\n"
     if colors is not None:
         colors = np.asarray(colors)
@@ -398,15 +399,17 @@ def write_ply(path, verts: np.ndarray, faces: np.ndarray, colors: np.ndarray | N
         vbytes = vrec.tobytes()
     else:
         vbytes = verts.tobytes()
-    header = ("ply\nformat binary_little_endian 1.0\n"
-              f"element vertex {len(verts)}\n{vprops}"
-              f"element face {len(faces)}\nproperty list uchar int vertex_indices\nend_header\n")
-    rec = np.empty(len(faces), dtype=[("n", "u1"), ("v", "<i4", (3,))])
-    rec["n"], rec["v"] = 3, faces
+    header = f"ply\nformat binary_little_endian 1.0\nelement vertex {len(verts)}\n{vprops}"
+    fbytes = b""
+    if faces is not None:
+        header += f"element face {len(faces)}\nproperty list uchar int vertex_indices\n"
+        rec = np.empty(len(faces), dtype=[("n", "u1"), ("v", "<i4", (3,))])
+        rec["n"], rec["v"] = 3, faces
+        fbytes = rec.tobytes()
     with open(path, "wb") as f:
-        f.write(header.encode("ascii"))
+        f.write((header + "end_header\n").encode("ascii"))
         f.write(vbytes)
-        f.write(rec.tobytes())
+        f.write(fbytes)
 
 
 _PLY_TYPES = {"char": "i1", "int8": "i1", "uchar": "u1", "uint8": "u1", "short": "<i2", "int16": "<i2",
