@@ -270,7 +270,9 @@ int32_t srcv_instnorm_to_chunk_planar_f32(const float* x, int32_t B, int32_t V, 
  *                              Z % 8 == 0 take the vector path; anything else a scalar path)
  *   origin                     world position of voxel (0,0,0) (fp32, TSDF.from_bounds :85)
  *   depth        DEVICE (B,H,W) fp16     cam_T_world, K  DEVICE (B,4,4) fp16
- *   depth_mask   DEVICE (B,H,W) uint8 (0 = invalid pixel, :251-253) or NULL             */
+ *   depth_mask   DEVICE (B,H,W) uint8 (0 = invalid pixel, :251-253) or NULL
+ * Limits (SRCV_ERR_SHAPE): B >= 1, 1 <= H, W <= 2048 (pixel coordinates exact in fp16), max_depth > min_depth.
+ * srcv_tsdf_workspace_bytes and srcv_sparse_tsdf_workspace_bytes are 0 for frame sizes outside them.      */
 typedef struct srcv_tsdf_volume {
   void* tsdf_values;
   void* tsdf_weights;
@@ -544,7 +546,8 @@ int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, doub
  *         (the caller inverts once per scan; the reference inverts per call, :25-27), all DEVICE
  *   pts_avg (H*W,3) out    n_valid (H*W) int32 out    valid (H*W) uint8 out (n_valid >= n_consistent)
  * The workspace keeps the staged per-frame matrices: pass frames_ready != 0 on every call after
- * the first of a scan to skip re-staging them.                                              */
+ * the first of a scan to skip re-staging them.  Limits (SRCV_ERR_SHAPE): N >= 1, H, W >= 2,
+ * H W <= 2^26, N H W <= 2^40; srcv_mvs_workspace_bytes is 0 outside them.                   */
 typedef struct srcv_mvs_scan {
   const float* depths;
   const float* K;
@@ -571,7 +574,9 @@ int32_t srcv_mvs_consistency_f32(const srcv_mvs_scan* scan, int32_t ref_index, f
  *           (B,K,H,W) float outputs = get_valid_mask of every view (NULL: not written).
  * backward: grad_depth_pred (B,1,H,W) out = grad_loss[0] * d loss / d depth_pred; `workspace` must
  *           be the one the forward call of the same arguments filled (it keeps the per-view counts).
- * Deterministic: per-CTA partial sums reduced in a fixed order.                                 */
+ * Deterministic: per-CTA partial sums reduced in a fixed order.
+ * Limits: B, K, H, W >= 1, B <= 65535, H W <= 2^26, B K H W <= 2^40 (SRCV_ERR_SHAPE) and K <= 16
+ * (SRCV_ERR_UNSUPPORTED); srcv_mvloss_workspace_bytes is 0 outside them.                         */
 typedef struct srcv_mvloss_args {
   const float* depth_pred;
   const float* cur_depth;

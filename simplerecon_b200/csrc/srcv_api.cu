@@ -44,6 +44,10 @@ static ProfRecord* prof_next() {
   return &g_prof[g_prof_used++];
 }
 
+// whether some pointer is not a multiple of `bytes` (a power of two); NULL counts as aligned
+template <class... P>
+static bool misaligned(uintptr_t bytes, const P*... p) { return ((reinterpret_cast<uintptr_t>(p) | ...) & (bytes - 1)) != 0; }
+
 static int32_t check_shape(const srcv_shape* s) {
   if (!s) return fail(SRCV_ERR_NULL, "shape is NULL");
   if (s->B <= 0 || s->K <= 0 || s->C <= 0 || s->H <= 0 || s->W <= 0 || s->D <= 0)
@@ -64,7 +68,7 @@ static int32_t check_common(const srcv_shape* s, const float* cur, const float* 
                             bool need_poses) {
   if (int32_t e = check_shape(s)) return e;
   if (!cur || !src || !cost) return fail(SRCV_ERR_NULL, "cur_feats/src_feats/cost is NULL");
-  if (((reinterpret_cast<uintptr_t>(cur) | reinterpret_cast<uintptr_t>(src)) & 15u) != 0)
+  if (misaligned(16, cur, src))
     return fail(SRCV_ERR_UNSUPPORTED, "cur_feats / src_feats must be 16-byte aligned");
   if (!cams || !cams->src_Ks || !cams->cur_invK) return fail(SRCV_ERR_NULL, "camera block incomplete");
   if (!cams->src_extrinsics) {
@@ -92,7 +96,7 @@ static int32_t check_common(const srcv_shape* s, const float* cur, const float* 
 
 static int32_t check_workspace(void* ws, size_t have, size_t need) {
   if (!ws) return fail(SRCV_ERR_NULL, "workspace is NULL (need %zu bytes)", need);
-  if ((reinterpret_cast<uintptr_t>(ws) & 255u) != 0)
+  if (misaligned(256, ws))
     return fail(SRCV_ERR_WORKSPACE, "workspace must be 256-byte aligned");
   if (have < need) return fail(SRCV_ERR_WORKSPACE, "workspace too small: %zu < %zu", have, need);
   return SRCV_OK;
@@ -103,6 +107,22 @@ static int32_t take_workspace(const srcv_shape& s, void* base, size_t have, bool
                               Workspace& ws) {
   if (int32_t e = check_workspace(base, have, carve_workspace(s, nullptr, want_c4, extra).bytes)) return e;
   ws = carve_workspace(s, base, want_c4, extra);
+  return SRCV_OK;
+}
+
+// An extract call's V / F against its buffers and the totals `count_call` left in the workspace (read back: a sync).
+template <class ReadTotals>
+static int32_t check_mesh_out(int64_t V, int64_t F, const float* verts, const int32_t* faces, const char* count_call,
+                              ReadTotals read_totals) {
+  if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
+  if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
+  if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
+  long long totals[2] = {-1, -1};
+  cudaError_t err = read_totals(totals);
+  if (err != cudaSuccess) return cuda_fail(err, "mesh totals");
+  if (totals[0] != V || totals[1] != F)
+    return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match %s (%lld, %lld) for this workspace", (long long)V,
+                (long long)F, count_call, totals[0], totals[1]);
   return SRCV_OK;
 }
 
@@ -164,8 +184,7 @@ const char* srcv_last_variant(void) { return g_last_variant.load(); }
 uint64_t srcv_launch_count(void) { return g_launches.load(); }
 
 size_t srcv_dot_workspace_bytes(const srcv_shape* s) {
-  if (check_shape(s) != SRCV_OK) return 0;
-  return carve_workspace(*s, nullptr, dot_fast_supported(*s), 0).bytes;
+  return check_shape(s) == SRCV_OK ? carve_workspace(*s, nullptr, dot_fast_supported(*s), 0).bytes : 0;
 }
 
 int32_t srcv_dot_forward_f32(const srcv_shape* s, const float* cur, const float* src,
@@ -202,8 +221,7 @@ int32_t srcv_dot_forward_f32(const srcv_shape* s, const float* cur, const float*
 }
 
 size_t srcv_dot_backward_workspace_bytes(const srcv_shape* s) {
-  if (check_shape(s) != SRCV_OK) return 0;
-  return carve_workspace(*s, nullptr, false, 0).bytes;
+  return check_shape(s) == SRCV_OK ? carve_workspace(*s, nullptr, false, 0).bytes : 0;
 }
 
 int32_t srcv_dot_backward_supported(const srcv_shape* s) {
@@ -234,8 +252,7 @@ int32_t srcv_dot_backward_f32(const srcv_shape* s, const float* cur, const float
 }
 
 size_t srcv_warp_workspace_bytes(const srcv_shape* s) {
-  if (check_shape(s) != SRCV_OK) return 0;
-  return carve_workspace(*s, nullptr, false, 0).bytes;
+  return check_shape(s) == SRCV_OK ? carve_workspace(*s, nullptr, false, 0).bytes : 0;
 }
 
 static int32_t warp_planes_impl(const srcv_shape* s, const float* src, const srcv_cameras* cams,
@@ -304,14 +321,12 @@ static size_t mlp_extra_bytes(const srcv_shape& s, const srcv_mlp_weights& w) {
 }
 
 size_t srcv_mlp_workspace_bytes(const srcv_shape* s, const srcv_mlp_weights* w) {
-  if (check_shape(s) != SRCV_OK || !w) return 0;
-  if (!mlp_generic_supported(*s, *w)) return 0;
+  if (check_shape(s) != SRCV_OK || !w || !mlp_generic_supported(*s, *w)) return 0;
   return carve_workspace(*s, nullptr, mlp_tc_supported(*s, *w), mlp_extra_bytes(*s, *w)).bytes;
 }
 
 size_t srcv_mlp_packed_bytes(const srcv_shape* s, const srcv_mlp_weights* w) {
-  if (check_shape(s) != SRCV_OK || !w) return 0;
-  return mlp_tc_supported(*s, *w) ? mlp_tc_image_bytes() : 0;
+  return check_shape(s) == SRCV_OK && w && mlp_tc_supported(*s, *w) ? mlp_tc_image_bytes() : 0;
 }
 
 int32_t srcv_mlp_pack_weights(const srcv_shape* s, const srcv_mlp_weights* w, void* image, void* stream_) {
@@ -320,7 +335,7 @@ int32_t srcv_mlp_pack_weights(const srcv_shape* s, const srcv_mlp_weights* w, vo
   if (!mlp_tc_supported(*s, *w))
     return fail(SRCV_ERR_UNSUPPORTED, "only the tensor-core variant (K == 7, C == 16, hidden 128/128) has a packed image");
   if (!image) return fail(SRCV_ERR_NULL, "image is NULL");
-  if ((reinterpret_cast<uintptr_t>(image) & 255u) != 0)
+  if (misaligned(256, image))
     return fail(SRCV_ERR_WORKSPACE, "image must be 256-byte aligned");
   cudaError_t err = launch_mlp_tc_pack(*w, image, static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "pack");
@@ -369,8 +384,7 @@ int32_t srcv_mlp_forward_f32(const srcv_shape* s, const float* cur, const float*
 }
 
 size_t srcv_mlp_backward_workspace_bytes(const srcv_shape* s, const srcv_mlp_weights* w) {
-  if (check_shape(s) != SRCV_OK || !w) return 0;
-  if (!mlp_backward_supported(*s, *w)) return 0;
+  if (check_shape(s) != SRCV_OK || !w || !mlp_backward_supported(*s, *w)) return 0;
   return carve_workspace(*s, nullptr, false, mlp_backward_extra_bytes(*s, *w)).bytes;
 }
 
@@ -426,7 +440,7 @@ int32_t srcv_instnorm_to_chunk_planar_f32(const float* x, int32_t B, int32_t V, 
       (long long)B * V * (C / 4) > 2147483647ll)
     return fail(SRCV_ERR_SHAPE, "bad shape B=%d V=%d C=%d H=%d W=%d (C must be a multiple of 4)", B, V, C, H, W);
   if (!(eps >= 0.f)) return fail(SRCV_ERR_SHAPE, "eps must be non-negative");
-  if (((reinterpret_cast<uintptr_t>(cur_c4) | reinterpret_cast<uintptr_t>(src_c4)) & 15u) != 0)
+  if (misaligned(16, cur_c4, src_c4))
     return fail(SRCV_ERR_UNSUPPORTED, "chunk-planar outputs must be 16-byte aligned");
   g_last_variant.store("instnorm_chunk_planar");
   cudaError_t err = launch_instnorm_c4(x, B, V, C, H, W, eps, cur_c4, src_c4, static_cast<cudaStream_t>(stream_));
@@ -434,28 +448,45 @@ int32_t srcv_instnorm_to_chunk_planar_f32(const float* x, int32_t B, int32_t V, 
   return SRCV_OK;
 }
 
+static bool tsdf_frames_dims_ok(const srcv_tsdf_frames* f) { return f->B > 0 && f->H > 0 && f->W > 0 && f->H <= 2048 && f->W <= 2048; }
+
+static int32_t check_frames(const srcv_tsdf_frames* f) {
+  if (!f) return fail(SRCV_ERR_NULL, "frames descriptor is NULL");
+  if (!f->depth || !f->cam_T_world || !f->K) return fail(SRCV_ERR_NULL, "depth / cam_T_world / K is NULL");
+  if (!tsdf_frames_dims_ok(f))
+    return fail(SRCV_ERR_SHAPE, "bad frame batch B=%d H=%d W=%d (image sizes up to 2048 are exact in fp16)", f->B, f->H, f->W);
+  if (!(f->max_depth > f->min_depth)) return fail(SRCV_ERR_SHAPE, "max_depth must exceed min_depth");
+  if (misaligned(2, f->depth, f->cam_T_world, f->K))
+    return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
+  return SRCV_OK;
+}
+
+static int32_t check_color_images(const srcv_tsdf_color* c) {
+  if (c->Hc < 1 || c->Wc < 1 || (long long)c->Hc * c->Wc > (1ll << 30))
+    return fail(SRCV_ERR_SHAPE, "bad colour image size Hc=%d Wc=%d", c->Hc, c->Wc);
+  for (int ch = 0; ch < 3; ++ch)
+    if (!(c->std[ch] != 0.f)) return fail(SRCV_ERR_SHAPE, "colour std[%d] must be non-zero", ch);
+  if (misaligned(4, c->images))
+    return fail(SRCV_ERR_UNSUPPORTED, "f32 colour arrays must be 4-byte aligned");
+  return SRCV_OK;
+}
+
 size_t srcv_tsdf_workspace_bytes(const srcv_tsdf_frames* f) {
-  if (!f || f->B <= 0) return 0;
-  return tsdf_workspace_bytes(f->B);
+  return f && tsdf_frames_dims_ok(f) ? tsdf_workspace_bytes(f->B) : 0;
 }
 
 static int32_t check_tsdf(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, void* workspace,
                           size_t workspace_bytes) {
   if (!v || !f) return fail(SRCV_ERR_NULL, "volume / frames descriptor is NULL");
   if (!v->tsdf_values || !v->tsdf_weights) return fail(SRCV_ERR_NULL, "tsdf_values / tsdf_weights is NULL");
-  if (!f->depth || !f->cam_T_world || !f->K) return fail(SRCV_ERR_NULL, "depth / cam_T_world / K is NULL");
+  if (int32_t e = check_frames(f)) return e;
   if (v->X <= 0 || v->Y <= 0 || v->Z <= 0 || (long long)v->X * v->Y * v->Z > (1ll << 40))
     return fail(SRCV_ERR_SHAPE, "bad volume dimensions %d x %d x %d", v->X, v->Y, v->Z);
-  if (f->B <= 0 || f->H <= 0 || f->W <= 0 || f->W > 2048 || f->H > 2048)
-    return fail(SRCV_ERR_SHAPE, "bad frame batch B=%d H=%d W=%d (image sizes up to 2048 are exact in fp16)", f->B, f->H, f->W);
-  if (!(v->voxel_size > 0.f) || !(v->truncation_voxels > 0.f) || !(v->max_weight > 0.f) || !(f->max_depth > f->min_depth))
-    return fail(SRCV_ERR_SHAPE, "voxel_size, truncation, max_weight must be positive and max_depth > min_depth");
-  if (((reinterpret_cast<uintptr_t>(v->tsdf_values) | reinterpret_cast<uintptr_t>(v->tsdf_weights) |
-        reinterpret_cast<uintptr_t>(f->depth) | reinterpret_cast<uintptr_t>(f->cam_T_world) |
-        reinterpret_cast<uintptr_t>(f->K)) & 1u) != 0)
+  if (!(v->voxel_size > 0.f) || !(v->truncation_voxels > 0.f) || !(v->max_weight > 0.f))
+    return fail(SRCV_ERR_SHAPE, "voxel_size, truncation, max_weight must be positive");
+  if (misaligned(2, v->tsdf_values, v->tsdf_weights))
     return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
-  if (int32_t e = check_workspace(workspace, workspace_bytes, tsdf_workspace_bytes(f->B))) return e;
-  return SRCV_OK;
+  return check_workspace(workspace, workspace_bytes, tsdf_workspace_bytes(f->B));
 }
 
 int32_t srcv_tsdf_integrate_f16(const srcv_tsdf_volume* v, const srcv_tsdf_frames* f, void* workspace,
@@ -472,11 +503,8 @@ int32_t srcv_tsdf_integrate_color_f16(const srcv_tsdf_volume* v, const srcv_tsdf
   if (!c) return fail(SRCV_ERR_NULL, "colour descriptor is NULL");
   if (!c->colors || !c->images) return fail(SRCV_ERR_NULL, "colors / images is NULL");
   if (int32_t e = check_tsdf(v, f, workspace, workspace_bytes)) return e;
-  if (c->Hc < 1 || c->Wc < 1 || (long long)c->Hc * c->Wc > (1ll << 30))
-    return fail(SRCV_ERR_SHAPE, "bad colour image size Hc=%d Wc=%d", c->Hc, c->Wc);
-  for (int ch = 0; ch < 3; ++ch)
-    if (!(c->std[ch] != 0.f)) return fail(SRCV_ERR_SHAPE, "colour std[%d] must be non-zero", ch);
-  if (((reinterpret_cast<uintptr_t>(c->colors) | reinterpret_cast<uintptr_t>(c->images)) & 3u) != 0)
+  if (int32_t e = check_color_images(c)) return e;
+  if (misaligned(4, c->colors))
     return fail(SRCV_ERR_UNSUPPORTED, "f32 colour arrays must be 4-byte aligned");
   g_last_variant.store("tsdf_integrate_color_f16");
   cudaError_t err = launch_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_), c);
@@ -484,23 +512,22 @@ int32_t srcv_tsdf_integrate_color_f16(const srcv_tsdf_volume* v, const srcv_tsdf
   return SRCV_OK;
 }
 
+static bool mesh_dims_ok(const srcv_mesh_args* a) { return a->X >= 2 && a->Y >= 2 && a->Z >= 2 && mesh_shape_supported(*a); }
+
 static int32_t check_mesh(const srcv_mesh_args* a) {
   if (!a) return fail(SRCV_ERR_NULL, "mesh arguments are NULL");
   if (!a->tsdf_values) return fail(SRCV_ERR_NULL, "tsdf_values is NULL");
   if (a->single_mesh && !a->tsdf_weights) return fail(SRCV_ERR_NULL, "single_mesh needs tsdf_weights");
-  if (a->X < 2 || a->Y < 2 || a->Z < 2)
-    return fail(SRCV_ERR_SHAPE, "bad volume dimensions %d x %d x %d (each must be >= 2)", a->X, a->Y, a->Z);
-  if (!mesh_shape_supported(*a))
-    return fail(SRCV_ERR_SHAPE, "volume %d x %d x %d out of range (X <= 65535, Y * Z < 2^31)", a->X, a->Y, a->Z);
+  if (!mesh_dims_ok(a))
+    return fail(SRCV_ERR_SHAPE, "bad volume dimensions %d x %d x %d (each >= 2, X <= 65535, Y * Z < 2^31)", a->X, a->Y, a->Z);
   if (a->scale_to_world && !(a->voxel_size > 0.f)) return fail(SRCV_ERR_SHAPE, "voxel_size must be positive");
-  if (((reinterpret_cast<uintptr_t>(a->tsdf_values) | reinterpret_cast<uintptr_t>(a->tsdf_weights)) & 1u) != 0)
+  if (misaligned(2, a->tsdf_values, a->tsdf_weights))
     return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
   return SRCV_OK;
 }
 
 size_t srcv_mesh_workspace_bytes(const srcv_mesh_args* a) {
-  if (!a || a->X < 2 || a->Y < 2 || a->Z < 2 || !mesh_shape_supported(*a)) return 0;
-  return mesh_workspace_bytes(*a);
+  return a && mesh_dims_ok(a) ? mesh_workspace_bytes(*a) : 0;
 }
 
 int32_t srcv_mesh_count(const srcv_mesh_args* a, int64_t* counts, void* workspace, size_t workspace_bytes,
@@ -518,19 +545,13 @@ int32_t srcv_mesh_count(const srcv_mesh_args* a, int64_t* counts, void* workspac
 static int32_t mesh_extract(const srcv_mesh_args* a, const float* colors, float* verts, float* normals,
                             float* vert_colors, int32_t* faces, int64_t V, int64_t F, void* workspace,
                             size_t workspace_bytes, void* stream_) {
-  if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
-  if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
-  if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
   if (int32_t e = check_workspace(workspace, workspace_bytes, mesh_workspace_bytes(*a))) return e;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  long long totals[2] = {-1, -1};
-  cudaError_t err = mesh_read_totals(*a, workspace, totals, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "mesh totals");
-  if (totals[0] != V || totals[1] != F)
-    return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match srcv_mesh_count (%lld, %lld) for this workspace",
-                (long long)V, (long long)F, totals[0], totals[1]);
+  if (int32_t e = check_mesh_out(V, F, verts, faces, "srcv_mesh_count",
+                                 [&](long long* t) { return mesh_read_totals(*a, workspace, t, stream); }))
+    return e;
   g_last_variant.store(colors ? "tsdf_mesh_mc_color" : "tsdf_mesh_mc");
-  err = launch_mesh_extract(*a, verts, normals, faces, workspace, stream, colors, vert_colors);
+  cudaError_t err = launch_mesh_extract(*a, verts, normals, faces, workspace, stream, colors, vert_colors);
   if (err != cudaSuccess) return cuda_fail(err, "mesh_extract");
   return SRCV_OK;
 }
@@ -548,25 +569,25 @@ int32_t srcv_mesh_extract_color(const srcv_mesh_args* a, const void* colors, flo
   if (!a->tsdf_weights) return fail(SRCV_ERR_NULL, "vertex colours need tsdf_weights");
   if (!colors) return fail(SRCV_ERR_NULL, "colors is NULL");
   if (V > 0 && !vert_colors) return fail(SRCV_ERR_NULL, "vert_colors is NULL");
-  if ((reinterpret_cast<uintptr_t>(colors) & 3u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "colors must be 4-byte aligned");
+  if (misaligned(4, colors)) return fail(SRCV_ERR_UNSUPPORTED, "colors must be 4-byte aligned");
   return mesh_extract(a, static_cast<const float*>(colors), verts, normals, vert_colors, faces, V, F, workspace,
                       workspace_bytes, stream_);
 }
 
+static bool sparse_dims_ok(const srcv_sparse_tsdf* v) { return v->max_blocks >= 1 && v->max_blocks <= (1 << 26); }
+
 static int32_t check_sparse(const srcv_sparse_tsdf* v) {
   if (!v) return fail(SRCV_ERR_NULL, "sparse volume descriptor is NULL");
   if (!v->state) return fail(SRCV_ERR_NULL, "state is NULL");
-  if (v->max_blocks < 1 || v->max_blocks > (1 << 26))
-    return fail(SRCV_ERR_SHAPE, "max_blocks = %d out of range (1 .. 2^26)", v->max_blocks);
+  if (!sparse_dims_ok(v)) return fail(SRCV_ERR_SHAPE, "max_blocks = %d out of range (1 .. 2^26)", v->max_blocks);
   if (!(v->voxel_size > 0.f) || !(v->truncation_voxels > 0.f) || !(v->max_weight > 0.f))
     return fail(SRCV_ERR_SHAPE, "voxel_size, truncation and max_weight must be positive");
-  if ((reinterpret_cast<uintptr_t>(v->state) & 255u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "state must be 256-byte aligned");
+  if (misaligned(256, v->state)) return fail(SRCV_ERR_UNSUPPORTED, "state must be 256-byte aligned");
   return SRCV_OK;
 }
 
 size_t srcv_sparse_tsdf_state_bytes(const srcv_sparse_tsdf* v) {
-  if (!v || v->max_blocks < 1 || v->max_blocks > (1 << 26)) return 0;
-  return sparse_tsdf_state_bytes(*v);
+  return v && sparse_dims_ok(v) ? sparse_tsdf_state_bytes(*v) : 0;
 }
 
 int32_t srcv_sparse_tsdf_reset(const srcv_sparse_tsdf* v, void* stream_) {
@@ -578,21 +599,13 @@ int32_t srcv_sparse_tsdf_reset(const srcv_sparse_tsdf* v, void* stream_) {
 }
 
 size_t srcv_sparse_tsdf_workspace_bytes(const srcv_tsdf_frames* f) {
-  if (!f || f->B <= 0 || f->H <= 0 || f->W <= 0) return 0;
-  return sparse_tsdf_workspace_bytes(*f);
+  return f && tsdf_frames_dims_ok(f) ? sparse_tsdf_workspace_bytes(*f) : 0;
 }
 
 static int32_t check_sparse_frames(const srcv_sparse_tsdf* v, const srcv_tsdf_frames* f, void* workspace,
                                    size_t workspace_bytes) {
   if (int32_t e = check_sparse(v)) return e;
-  if (!f) return fail(SRCV_ERR_NULL, "frames descriptor is NULL");
-  if (!f->depth || !f->cam_T_world || !f->K) return fail(SRCV_ERR_NULL, "depth / cam_T_world / K is NULL");
-  if (f->B <= 0 || f->H <= 0 || f->W <= 0 || f->W > 2048 || f->H > 2048)
-    return fail(SRCV_ERR_SHAPE, "bad frame batch B=%d H=%d W=%d (image sizes up to 2048 are exact in fp16)", f->B, f->H, f->W);
-  if (!(f->max_depth > f->min_depth)) return fail(SRCV_ERR_SHAPE, "max_depth must exceed min_depth");
-  if (((reinterpret_cast<uintptr_t>(f->depth) | reinterpret_cast<uintptr_t>(f->cam_T_world) |
-        reinterpret_cast<uintptr_t>(f->K)) & 1u) != 0)
-    return fail(SRCV_ERR_UNSUPPORTED, "fp16 arrays must be 2-byte aligned");
+  if (int32_t e = check_frames(f)) return e;
   return check_workspace(workspace, workspace_bytes, sparse_tsdf_workspace_bytes(*f));
 }
 
@@ -612,11 +625,7 @@ int32_t srcv_sparse_tsdf_integrate_color_f16(const srcv_sparse_tsdf* v, const sr
   if (!c->images) return fail(SRCV_ERR_NULL, "images is NULL");
   if (int32_t e = check_sparse_frames(v, f, workspace, workspace_bytes)) return e;
   if (!v->color) return fail(SRCV_ERR_UNSUPPORTED, "this sparse volume has no colour planes");
-  if (c->Hc < 1 || c->Wc < 1 || (long long)c->Hc * c->Wc > (1ll << 30))
-    return fail(SRCV_ERR_SHAPE, "bad colour image size Hc=%d Wc=%d", c->Hc, c->Wc);
-  for (int ch = 0; ch < 3; ++ch)
-    if (!(c->std[ch] != 0.f)) return fail(SRCV_ERR_SHAPE, "colour std[%d] must be non-zero", ch);
-  if ((reinterpret_cast<uintptr_t>(c->images) & 3u) != 0) return fail(SRCV_ERR_UNSUPPORTED, "images must be 4-byte aligned");
+  if (int32_t e = check_color_images(c)) return e;
   g_last_variant.store("sparse_tsdf_integrate_color_f16");
   cudaError_t err = launch_sparse_tsdf_integrate(*v, *f, workspace, static_cast<cudaStream_t>(stream_), c);
   if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_integrate_color");
@@ -640,16 +649,17 @@ int32_t srcv_sparse_tsdf_mesh_end(const srcv_sparse_tsdf* v, int32_t blocks, voi
   return SRCV_OK;
 }
 
+static bool sparse_mesh_dims_ok(const srcv_sparse_mesh_args* a) { return a->blocks >= 0; }
+
 size_t srcv_sparse_tsdf_mesh_workspace_bytes(const srcv_sparse_mesh_args* a) {
-  if (!a || a->blocks < 0) return 0;
-  return sparse_mesh_workspace_bytes(*a);
+  return a && sparse_mesh_dims_ok(a) ? sparse_mesh_workspace_bytes(*a) : 0;
 }
 
 static int32_t check_sparse_mesh(const srcv_sparse_tsdf* v, const srcv_sparse_mesh_args* a, void* workspace,
                                  size_t workspace_bytes) {
   if (int32_t e = check_sparse(v)) return e;
   if (!a) return fail(SRCV_ERR_NULL, "mesh arguments are NULL");
-  if (a->blocks < 0 || a->blocks > v->max_blocks)
+  if (!sparse_mesh_dims_ok(a) || a->blocks > v->max_blocks)
     return fail(SRCV_ERR_SHAPE, "blocks = %d outside 0 .. max_blocks = %d", a->blocks, v->max_blocks);
   return check_workspace(workspace, workspace_bytes, sparse_mesh_workspace_bytes(*a));
 }
@@ -669,19 +679,13 @@ int32_t srcv_sparse_tsdf_mesh_extract(const srcv_sparse_tsdf* v, const srcv_spar
                                       float* normals, float* vert_colors, int32_t* faces, int64_t V, int64_t F,
                                       void* workspace, size_t workspace_bytes, void* stream_) {
   if (int32_t e = check_sparse_mesh(v, a, workspace, workspace_bytes)) return e;
-  if (V < 0 || F < 0) return fail(SRCV_ERR_SHAPE, "negative V / F");
-  if (V > 2147483647ll) return fail(SRCV_ERR_UNSUPPORTED, "%lld vertices overflow the int32 face indices", (long long)V);
-  if ((V > 0 && !verts) || (F > 0 && !faces)) return fail(SRCV_ERR_NULL, "verts / faces is NULL");
   if (vert_colors && !v->color) return fail(SRCV_ERR_UNSUPPORTED, "vertex colours need a volume with colour planes");
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  long long totals[2] = {-1, -1};
-  cudaError_t err = sparse_mesh_read_totals(*a, workspace, totals, stream);
-  if (err != cudaSuccess) return cuda_fail(err, "sparse mesh totals");
-  if (totals[0] != V || totals[1] != F)
-    return fail(SRCV_ERR_SHAPE, "V=%lld F=%lld do not match srcv_sparse_tsdf_mesh_count (%lld, %lld) for this workspace",
-                (long long)V, (long long)F, totals[0], totals[1]);
+  if (int32_t e = check_mesh_out(V, F, verts, faces, "srcv_sparse_tsdf_mesh_count",
+                                 [&](long long* t) { return sparse_mesh_read_totals(*a, workspace, t, stream); }))
+    return e;
   g_last_variant.store(vert_colors ? "sparse_tsdf_mesh_mc_color" : "sparse_tsdf_mesh_mc");
-  err = launch_sparse_mesh_extract(*v, *a, verts, normals, vert_colors, faces, workspace, stream);
+  cudaError_t err = launch_sparse_mesh_extract(*v, *a, verts, normals, vert_colors, faces, workspace, stream);
   if (err != cudaSuccess) return cuda_fail(err, "sparse_tsdf_mesh_extract");
   return SRCV_OK;
 }
@@ -696,8 +700,7 @@ int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* v, const int32_t lo[3]
   for (int a = 0; a < 3; ++a)
     if ((long long)lo[a] < -(8ll << 20) || (long long)lo[a] + dims[a] > (8ll << 20))
       return fail(SRCV_ERR_SHAPE, "box outside the +-2^23-voxel lattice");
-  if (((reinterpret_cast<uintptr_t>(values) | reinterpret_cast<uintptr_t>(weights)) & 1u) != 0 ||
-      (reinterpret_cast<uintptr_t>(colors) & 3u) != 0)
+  if (misaligned(2, values, weights) || misaligned(4, colors))
     return fail(SRCV_ERR_UNSUPPORTED, "misaligned output arrays");
   g_last_variant.store("sparse_tsdf_read_box");
   cudaError_t err = launch_sparse_tsdf_read_box(*v, lo, dims, values, weights, colors, static_cast<cudaStream_t>(stream_));
@@ -707,9 +710,19 @@ int32_t srcv_sparse_tsdf_read_box(const srcv_sparse_tsdf* v, const int32_t lo[3]
 
 static constexpr long long kMeshEvalMaxPoints = 1ll << 28;   // ~25 GB of workspace at the limit
 
+static bool point_count_ok(int64_t n) { return n >= 1 && n <= kMeshEvalMaxPoints; }
+
 static bool mesh_eval_dims_ok(const srcv_mesh_eval_args* a) {
   return a->num_faces >= 0 && a->num_faces <= 2147483647ll && a->num_queries >= 0 &&
          a->num_queries <= kMeshEvalMaxPoints && a->num_points >= 0 && a->num_points <= kMeshEvalMaxPoints;
+}
+
+static int32_t check_flags(const srcv_mesh_eval_args* a) {
+  if (!a) return fail(SRCV_ERR_NULL, "mesh-evaluation arguments are NULL");
+  if (!a->flags) return fail(SRCV_ERR_NULL, "flags is NULL");
+  if (misaligned(4, a->flags) || misaligned(8, a->stats))
+    return fail(SRCV_ERR_UNSUPPORTED, "flags / stats misaligned");
+  return SRCV_OK;
 }
 
 // the distance and metric calls, and the compaction of num_points observed points
@@ -720,18 +733,14 @@ static size_t mesh_eval_all_workspace_bytes(const srcv_mesh_eval_args& a) {
 }
 
 size_t srcv_mesh_eval_workspace_bytes(const srcv_mesh_eval_args* a) {
-  if (!a || !mesh_eval_dims_ok(a)) return 0;
-  return mesh_eval_all_workspace_bytes(*a);
+  return a && mesh_eval_dims_ok(a) ? mesh_eval_all_workspace_bytes(*a) : 0;
 }
 
 static int32_t check_mesh_eval(const srcv_mesh_eval_args* a, void* workspace, size_t workspace_bytes) {
-  if (!a) return fail(SRCV_ERR_NULL, "mesh-evaluation arguments are NULL");
-  if (!a->flags) return fail(SRCV_ERR_NULL, "flags is NULL");
+  if (int32_t e = check_flags(a)) return e;
   if (!mesh_eval_dims_ok(a))
     return fail(SRCV_ERR_SHAPE, "bad sizes num_faces=%lld num_queries=%lld num_points=%lld (points at most 2^28)",
                 (long long)a->num_faces, (long long)a->num_queries, (long long)a->num_points);
-  if ((reinterpret_cast<uintptr_t>(a->flags) & 3u) != 0 || (reinterpret_cast<uintptr_t>(a->stats) & 7u) != 0)
-    return fail(SRCV_ERR_UNSUPPORTED, "flags / stats misaligned");
   return check_workspace(workspace, workspace_bytes, mesh_eval_workspace_bytes(*a));
 }
 
@@ -740,11 +749,10 @@ int32_t srcv_mesh_sample_f32(const srcv_mesh_eval_args* a, const float* verts, i
                              void* stream_) {
   if (int32_t e = check_mesh_eval(a, workspace, workspace_bytes)) return e;
   if (!verts || !faces || !samples) return fail(SRCV_ERR_NULL, "verts / faces / samples is NULL");
-  if (a->num_faces < 1 || V < 1 || num_samples < 1 || num_samples > kMeshEvalMaxPoints)
+  if (a->num_faces < 1 || V < 1 || !point_count_ok(num_samples))
     return fail(SRCV_ERR_SHAPE, "empty mesh or bad sample count: V=%d F=%lld num_samples=%lld", V,
                 (long long)a->num_faces, (long long)num_samples);
-  if (((reinterpret_cast<uintptr_t>(verts) | reinterpret_cast<uintptr_t>(faces) | reinterpret_cast<uintptr_t>(samples)) &
-       3u) != 0)
+  if (misaligned(4, verts, faces, samples))
     return fail(SRCV_ERR_UNSUPPORTED, "verts / faces / samples must be 4-byte aligned");
   g_last_variant.store("mesh_sample_f32");
   cudaError_t err = launch_mesh_sample(*a, verts, V, faces, num_samples, seed, samples, workspace,
@@ -760,8 +768,7 @@ int32_t srcv_nearest_distances_f32(const srcv_mesh_eval_args* a, const float* qu
   if (a->num_queries < 1 || a->num_points < 1)
     return fail(SRCV_ERR_SHAPE, "empty point set: num_queries=%lld num_points=%lld", (long long)a->num_queries,
                 (long long)a->num_points);
-  if (((reinterpret_cast<uintptr_t>(queries) | reinterpret_cast<uintptr_t>(points)) & 3u) != 0 ||
-      (reinterpret_cast<uintptr_t>(dist) & 7u) != 0)
+  if (misaligned(4, queries, points) || misaligned(8, dist))
     return fail(SRCV_ERR_UNSUPPORTED, "queries / points must be 4-byte and dist 8-byte aligned");
   g_last_variant.store("nearest_distances_f32");
   cudaError_t err = launch_nearest_distances(*a, queries, points, dist, workspace, static_cast<cudaStream_t>(stream_));
@@ -778,8 +785,7 @@ int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* a, const double* dist_p
     return fail(SRCV_ERR_SHAPE, "empty point set: |P|=%lld |G|=%lld", (long long)a->num_queries,
                 (long long)a->num_points);
   if (!(threshold > 0.0)) return fail(SRCV_ERR_SHAPE, "threshold must be positive");
-  if (((reinterpret_cast<uintptr_t>(dist_pred) | reinterpret_cast<uintptr_t>(dist_gt) |
-        reinterpret_cast<uintptr_t>(metrics)) & 7u) != 0)
+  if (misaligned(8, dist_pred, dist_gt, metrics))
     return fail(SRCV_ERR_UNSUPPORTED, "f64 arrays must be 8-byte aligned");
   g_last_variant.store("mesh_metrics_f64");
   cudaError_t err = launch_mesh_metrics(*a, dist_pred, dist_gt, threshold, metrics, workspace,
@@ -789,12 +795,9 @@ int32_t srcv_mesh_metrics_f64(const srcv_mesh_eval_args* a, const double* dist_p
 }
 
 static int32_t check_observed_points(const srcv_mesh_eval_args* a) {
-  if (!a) return fail(SRCV_ERR_NULL, "mesh-evaluation arguments are NULL");
-  if (!a->flags) return fail(SRCV_ERR_NULL, "flags is NULL");
-  if (a->num_points < 1 || a->num_points > kMeshEvalMaxPoints)
+  if (int32_t e = check_flags(a)) return e;
+  if (!point_count_ok(a->num_points))
     return fail(SRCV_ERR_SHAPE, "bad point count num_points=%lld (1 .. 2^28)", (long long)a->num_points);
-  if ((reinterpret_cast<uintptr_t>(a->flags) & 3u) != 0 || (reinterpret_cast<uintptr_t>(a->stats) & 7u) != 0)
-    return fail(SRCV_ERR_UNSUPPORTED, "flags / stats misaligned");
   return SRCV_OK;
 }
 
@@ -809,9 +812,7 @@ int32_t srcv_observation_counts_f32(const srcv_mesh_eval_args* a, const srcv_mes
   if (!(v->margin >= 0.0 && std::isfinite(v->margin)) || !(v->max_depth > 0.0))
     return fail(SRCV_ERR_SHAPE, "margin must be finite and >= 0, max_depth > 0 (margin=%g max_depth=%g)", v->margin,
                 v->max_depth);
-  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(counts) |
-        reinterpret_cast<uintptr_t>(v->depths) | reinterpret_cast<uintptr_t>(v->K) |
-        reinterpret_cast<uintptr_t>(v->cam_T_world)) & 3u) != 0)
+  if (misaligned(4, points, counts, v->depths, v->K, v->cam_T_world))
     return fail(SRCV_ERR_UNSUPPORTED, "points / counts / depths / K / cam_T_world must be 4-byte aligned");
   g_last_variant.store("observation_counts_f32");
   cudaError_t err = launch_observation_counts(*a, *v, points, counts, static_cast<cudaStream_t>(stream_));
@@ -823,8 +824,7 @@ int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* a, const float* poi
                                   int64_t* num_kept, void* workspace, size_t workspace_bytes, void* stream_) {
   if (int32_t e = check_observed_points(a)) return e;
   if (!points || !counts || !kept || !num_kept) return fail(SRCV_ERR_NULL, "points / counts / kept / num_kept is NULL");
-  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(counts) | reinterpret_cast<uintptr_t>(kept)) &
-       3u) != 0 || (reinterpret_cast<uintptr_t>(num_kept) & 7u) != 0)
+  if (misaligned(4, points, counts, kept) || misaligned(8, num_kept))
     return fail(SRCV_ERR_UNSUPPORTED, "points / counts / kept must be 4-byte and num_kept 8-byte aligned");
   if (int32_t e = check_workspace(workspace, workspace_bytes, observed_compact_workspace_bytes(a->num_points))) return e;
   g_last_variant.store("compact_observed_f32");
@@ -835,8 +835,7 @@ int32_t srcv_compact_observed_f32(const srcv_mesh_eval_args* a, const float* poi
 }
 
 size_t srcv_voxel_down_sample_workspace_bytes(int64_t num_points) {
-  if (num_points < 1 || num_points > kMeshEvalMaxPoints) return 0;
-  return voxel_down_sample_workspace_bytes(num_points);
+  return point_count_ok(num_points) ? voxel_down_sample_workspace_bytes(num_points) : 0;
 }
 
 int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, double voxel_size, const void* colors,
@@ -845,7 +844,7 @@ int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, doub
                                    void* stream_) {
   if (!points || !out_points || !out_counts || !num_out || !flags)
     return fail(SRCV_ERR_NULL, "points / out_points / out_counts / num_out / flags is NULL");
-  if (num_points < 1 || num_points > kMeshEvalMaxPoints)
+  if (!point_count_ok(num_points))
     return fail(SRCV_ERR_SHAPE, "bad point count num_points=%lld (1 .. 2^28)", (long long)num_points);
   if (!(voxel_size > 0.0 && std::isfinite(voxel_size)))
     return fail(SRCV_ERR_SHAPE, "voxel_size must be finite and > 0, got %g", voxel_size);
@@ -854,10 +853,8 @@ int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, doub
   if ((color_type != SRCV_COLORS_NONE) != (colors != nullptr && out_colors != nullptr))
     return fail(SRCV_ERR_NULL, "colors and out_colors must be given exactly when color_type is not SRCV_COLORS_NONE");
   const uintptr_t csize = color_type == SRCV_COLORS_F64 ? 8u : color_type == SRCV_COLORS_F32 ? 4u : 1u;
-  if (((reinterpret_cast<uintptr_t>(points) | reinterpret_cast<uintptr_t>(out_points) |
-        reinterpret_cast<uintptr_t>(out_colors) | reinterpret_cast<uintptr_t>(out_counts) |
-        reinterpret_cast<uintptr_t>(flags)) & 3u) != 0 || (reinterpret_cast<uintptr_t>(num_out) & 7u) != 0 ||
-      (reinterpret_cast<uintptr_t>(colors) & (csize - 1u)) != 0)
+  if (misaligned(4, points, out_points, out_colors, out_counts, flags) || misaligned(8, num_out) ||
+      misaligned(csize, colors))
     return fail(SRCV_ERR_UNSUPPORTED, "misaligned point, colour, count or flag arrays");
   if (int32_t e = check_workspace(workspace, workspace_bytes, voxel_down_sample_workspace_bytes(num_points))) return e;
   g_last_variant.store("voxel_down_sample_f32");
@@ -867,9 +864,13 @@ int32_t srcv_voxel_down_sample_f32(const float* points, int64_t num_points, doub
   return SRCV_OK;
 }
 
+static bool mvs_dims_ok(const srcv_mvs_scan* s) {
+  return s->N > 0 && s->H > 1 && s->W > 1 && (long long)s->H * s->W <= (1ll << 26) &&
+         (long long)s->N * s->H * s->W <= (1ll << 40);
+}
+
 size_t srcv_mvs_workspace_bytes(const srcv_mvs_scan* s) {
-  if (!s || s->N <= 0) return 0;
-  return mvs_workspace_bytes(s->N);
+  return s && mvs_dims_ok(s) ? mvs_workspace_bytes(s->N) : 0;
 }
 
 int32_t srcv_mvs_consistency_f32(const srcv_mvs_scan* s, int32_t ref, float z_thresh, int32_t n_consistent,
@@ -879,9 +880,7 @@ int32_t srcv_mvs_consistency_f32(const srcv_mvs_scan* s, int32_t ref, float z_th
   if (!s->depths || !s->K || !s->K_inv || !s->cam_T_world || !s->world_T_cam)
     return fail(SRCV_ERR_NULL, "a scan pointer is NULL");
   if (!pts_avg || !n_valid || !valid) return fail(SRCV_ERR_NULL, "an output pointer is NULL");
-  if (s->N <= 0 || s->H <= 1 || s->W <= 1 || (long long)s->H * s->W > (1ll << 26) ||
-      (long long)s->N * s->H * s->W > (1ll << 40))
-    return fail(SRCV_ERR_SHAPE, "bad scan shape N=%d H=%d W=%d", s->N, s->H, s->W);
+  if (!mvs_dims_ok(s)) return fail(SRCV_ERR_SHAPE, "bad scan shape N=%d H=%d W=%d", s->N, s->H, s->W);
   if (ref < 0 || ref >= s->N) return fail(SRCV_ERR_SHAPE, "ref_index %d out of range [0,%d)", ref, s->N);
   if (int32_t e = check_workspace(workspace, workspace_bytes, mvs_workspace_bytes(s->N))) return e;
   g_last_variant.store("mvs_consistency_f32");
@@ -891,29 +890,31 @@ int32_t srcv_mvs_consistency_f32(const srcv_mvs_scan* s, int32_t ref, float z_th
   return SRCV_OK;
 }
 
-static int32_t check_mvloss(const srcv_mvloss_args* a) {
+static bool mvloss_dims_ok(const srcv_mvloss_args* a) {
+  return a->B > 0 && a->K > 0 && a->H > 0 && a->W > 0 && (long long)a->H * a->W <= (1ll << 26) &&
+         (long long)a->B * a->K * a->H * a->W <= (1ll << 40) && a->B <= 65535 && a->K <= mvloss_max_views();
+}
+
+static int32_t check_mvloss(const srcv_mvloss_args* a, const void* workspace, size_t workspace_bytes) {
   if (!a) return fail(SRCV_ERR_NULL, "loss arguments are NULL");
   if (!a->depth_pred || !a->cur_depth || !a->src_depth || !a->cur_invK || !a->src_K || !a->cur_world_T_cam ||
       !a->src_cam_T_world)
     return fail(SRCV_ERR_NULL, "a loss input pointer is NULL");
-  if (a->B <= 0 || a->K <= 0 || a->H <= 0 || a->W <= 0 || (long long)a->H * a->W > (1ll << 26) ||
-      (long long)a->B * a->K * a->H * a->W > (1ll << 40) || a->B > 65535)
-    return fail(SRCV_ERR_SHAPE, "bad loss shape B=%d K=%d H=%d W=%d", a->B, a->K, a->H, a->W);
-  if (a->K > mvloss_max_views())
-    return fail(SRCV_ERR_UNSUPPORTED, "at most %d source views per call (got %d)", mvloss_max_views(), a->K);
-  return SRCV_OK;
+  if (!mvloss_dims_ok(a))   // too many views is a limit of this build's kernels, not a malformed shape
+    return a->K > mvloss_max_views()
+               ? fail(SRCV_ERR_UNSUPPORTED, "at most %d source views per call (got %d)", mvloss_max_views(), a->K)
+               : fail(SRCV_ERR_SHAPE, "bad loss shape B=%d K=%d H=%d W=%d", a->B, a->K, a->H, a->W);
+  return check_workspace(const_cast<void*>(workspace), workspace_bytes, mvloss_workspace_bytes(*a));
 }
 
 size_t srcv_mvloss_workspace_bytes(const srcv_mvloss_args* a) {
-  if (!a || a->B <= 0 || a->K <= 0 || a->H <= 0 || a->W <= 0) return 0;
-  return mvloss_workspace_bytes(*a);
+  return a && mvloss_dims_ok(a) ? mvloss_workspace_bytes(*a) : 0;
 }
 
 int32_t srcv_mvloss_forward_f32(const srcv_mvloss_args* a, float* loss, uint8_t* valid_mask, float* sampled,
                                 void* workspace, size_t workspace_bytes, void* stream_) {
-  if (int32_t e = check_mvloss(a)) return e;
   if (!loss) return fail(SRCV_ERR_NULL, "loss output pointer is NULL");
-  if (int32_t e = check_workspace(workspace, workspace_bytes, mvloss_workspace_bytes(*a))) return e;
+  if (int32_t e = check_mvloss(a, workspace, workspace_bytes)) return e;
   g_last_variant.store("mvloss_forward_f32");
   cudaError_t err = launch_mvloss_forward(*a, loss, valid_mask, sampled, workspace, static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "mvloss_forward");
@@ -922,9 +923,8 @@ int32_t srcv_mvloss_forward_f32(const srcv_mvloss_args* a, float* loss, uint8_t*
 
 int32_t srcv_mvloss_backward_f32(const srcv_mvloss_args* a, const float* grad_loss, float* grad_depth_pred,
                                  const void* workspace, size_t workspace_bytes, void* stream_) {
-  if (int32_t e = check_mvloss(a)) return e;
   if (!grad_loss || !grad_depth_pred) return fail(SRCV_ERR_NULL, "grad_loss / grad_depth_pred is NULL");
-  if (int32_t e = check_workspace(const_cast<void*>(workspace), workspace_bytes, mvloss_workspace_bytes(*a))) return e;
+  if (int32_t e = check_mvloss(a, workspace, workspace_bytes)) return e;
   g_last_variant.store("mvloss_backward_f32");
   cudaError_t err = launch_mvloss_backward(*a, grad_loss, grad_depth_pred, workspace, static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "mvloss_backward");
@@ -936,8 +936,7 @@ static bool metrics_dims_ok(const srcv_metrics_args* a) {
 }
 
 size_t srcv_metrics_workspace_bytes(const srcv_metrics_args* a) {
-  if (!a || !metrics_dims_ok(a)) return 0;
-  return metrics_workspace_bytes(*a);
+  return a && metrics_dims_ok(a) ? metrics_workspace_bytes(*a) : 0;
 }
 
 int32_t srcv_depth_metrics_f32(const srcv_metrics_args* a, float* metrics, int64_t* valid_counts, float* upsampled,
@@ -990,8 +989,7 @@ static int32_t check_normals(const srcv_normals_args* a) {
 }
 
 size_t srcv_normals_workspace_bytes(const srcv_normals_args* a) {
-  if (!a || !normals_dims_ok(a)) return 0;
-  return normals_workspace_bytes(*a);
+  return a && normals_dims_ok(a) ? normals_workspace_bytes(*a) : 0;
 }
 
 int32_t srcv_normals_forward_f32(const srcv_normals_args* a, float* normals, void* stream_) {
@@ -1018,17 +1016,20 @@ static bool normals_loss_dims_ok(int32_t B, int32_t H, int32_t W) {
   return B >= 1 && H >= 1 && W >= 1 && 3ll * B * H * W < (1ll << 31);
 }
 
+static int32_t check_normals_loss(int32_t B, int32_t H, int32_t W, const void* workspace, size_t workspace_bytes) {
+  if (!normals_loss_dims_ok(B, H, W))
+    return fail(SRCV_ERR_SHAPE, "bad normals-loss shape B=%d H=%d W=%d (3 B H W < 2^31)", B, H, W);
+  return check_workspace(const_cast<void*>(workspace), workspace_bytes, normals_loss_workspace_bytes(B, H, W));
+}
+
 size_t srcv_normals_loss_workspace_bytes(int32_t B, int32_t H, int32_t W) {
-  if (!normals_loss_dims_ok(B, H, W)) return 0;
-  return normals_loss_workspace_bytes(B, H, W);
+  return normals_loss_dims_ok(B, H, W) ? normals_loss_workspace_bytes(B, H, W) : 0;
 }
 
 int32_t srcv_normals_loss_forward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W, float* loss,
                                       void* workspace, size_t workspace_bytes, void* stream_) {
   if (!gt || !pred || !loss) return fail(SRCV_ERR_NULL, "normals_gt / normals_pred / loss is NULL");
-  if (!normals_loss_dims_ok(B, H, W))
-    return fail(SRCV_ERR_SHAPE, "bad normals-loss shape B=%d H=%d W=%d (3 B H W < 2^31)", B, H, W);
-  if (int32_t e = check_workspace(workspace, workspace_bytes, normals_loss_workspace_bytes(B, H, W))) return e;
+  if (int32_t e = check_normals_loss(B, H, W, workspace, workspace_bytes)) return e;
   g_last_variant.store("normals_loss_forward_f32");
   cudaError_t err = launch_normals_loss_forward(gt, pred, B, H, W, loss, workspace, static_cast<cudaStream_t>(stream_));
   if (err != cudaSuccess) return cuda_fail(err, "normals_loss_forward");
@@ -1040,10 +1041,7 @@ int32_t srcv_normals_loss_backward_f32(const float* gt, const float* pred, int32
                                        const void* workspace, size_t workspace_bytes, void* stream_) {
   if (!gt || !pred || !grad_loss || !grad_pred)
     return fail(SRCV_ERR_NULL, "normals_gt / normals_pred / grad_loss / grad_pred is NULL");
-  if (!normals_loss_dims_ok(B, H, W))
-    return fail(SRCV_ERR_SHAPE, "bad normals-loss shape B=%d H=%d W=%d (3 B H W < 2^31)", B, H, W);
-  if (int32_t e = check_workspace(const_cast<void*>(workspace), workspace_bytes, normals_loss_workspace_bytes(B, H, W)))
-    return e;
+  if (int32_t e = check_normals_loss(B, H, W, workspace, workspace_bytes)) return e;
   g_last_variant.store("normals_loss_backward_f32");
   cudaError_t err = launch_normals_loss_backward(gt, pred, B, H, W, grad_loss, grad_pred, grad_gt, workspace,
                                                  static_cast<cudaStream_t>(stream_));
@@ -1066,8 +1064,7 @@ static int32_t check_msgrad(const float* gt, const float* pred, int32_t B, int32
 }
 
 size_t srcv_msgrad_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t num_scales) {
-  if (!msgrad_dims_ok(B, H, W, num_scales)) return 0;
-  return msgrad_workspace_bytes(B, H, W, num_scales);
+  return msgrad_dims_ok(B, H, W, num_scales) ? msgrad_workspace_bytes(B, H, W, num_scales) : 0;
 }
 
 int32_t srcv_msgrad_forward_f32(const float* gt, const float* pred, int32_t B, int32_t H, int32_t W, int32_t num_scales,
@@ -1093,16 +1090,17 @@ int32_t srcv_msgrad_backward_f32(const float* gt, const float* pred, int32_t B, 
   return SRCV_OK;
 }
 
+static bool si_loss_dims_ok(int64_t n) { return n >= 0 && n < (1ll << 31); }
+
 static int32_t check_si_loss(const float* gt, const float* pred, int64_t n, const void* workspace,
                              size_t workspace_bytes) {
-  if (n < 0 || n >= (1ll << 31)) return fail(SRCV_ERR_SHAPE, "bad scale-invariant loss size n=%lld (0 <= n < 2^31)", (long long)n);
+  if (!si_loss_dims_ok(n)) return fail(SRCV_ERR_SHAPE, "bad scale-invariant loss size n=%lld (0 <= n < 2^31)", (long long)n);
   if (n > 0 && (!gt || !pred)) return fail(SRCV_ERR_NULL, "log_depth_gt / log_depth_pred is NULL");
   return check_workspace(const_cast<void*>(workspace), workspace_bytes, si_loss_workspace_bytes(n));
 }
 
 size_t srcv_si_loss_workspace_bytes(int64_t n) {
-  if (n < 0 || n >= (1ll << 31)) return 0;
-  return si_loss_workspace_bytes(n);
+  return si_loss_dims_ok(n) ? si_loss_workspace_bytes(n) : 0;
 }
 
 int32_t srcv_si_loss_forward_f32(const float* gt, const float* pred, int64_t n, double si_lambda, float* loss,
@@ -1148,8 +1146,7 @@ static int32_t check_regloss(const srcv_regloss_args* a, const void* workspace, 
 }
 
 size_t srcv_regloss_workspace_bytes(const srcv_regloss_args* a) {
-  if (!a || !a->log_pred[0] || !regloss_dims_ok(a)) return 0;
-  return regloss_workspace_bytes(*a);
+  return a && a->log_pred[0] && regloss_dims_ok(a) ? regloss_workspace_bytes(*a) : 0;
 }
 
 int32_t srcv_regloss_forward_f32(const srcv_regloss_args* a, float* losses, void* workspace, size_t workspace_bytes,
